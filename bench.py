@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- agent-steps/sec of the RatInABox per-step hot path on B200.
+"""bench.py -- agent-steps/sec of the RatInABox per-step hot path on H100.
 
 One "step" = Agent.update() + Neurons.update() of every population for every agent
 (BASELINE.json metric).  Default workload = BASELINE.json configs[1]:
@@ -8,6 +8,7 @@ reference's default wall geometry for that box (geodesic -> line_of_sight,
 ratinabox/Neurons.py:922-928), dt = 10 ms, history + spikes on (reference defaults).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c2e|c3|c4]
+                  [--dump-outputs DIR]
 
 N > 1 is launched by torchrun (one rank per GPU); agents are sharded (weak scaling:
 65 536 agents per GPU), there is no collective on the step path.
@@ -270,10 +271,40 @@ def algorithmic_bytes_per_agent_step(n_cells, spikes):
     return 2 * 12 * 8 + 8 * 4 + 4 * n_cells + (n_cells // 8 if spikes else 0)
 
 
+DUMP_AGENTS = 4096          # --dump-outputs: fixed, seeded sample of agents (the full rate rows of c2 are 268 MB)
+DUMP_BYTES_MAX = 64 << 20
+
+
+def dump_outputs(torch, Ag, pops, out_dir):
+    """What the timed riab_run computed in its last step, for a fixed seeded sample of agents: every agent state array
+    (float64) and, per population k, the rate row (float32) and the spikes (0/1 as float32)."""
+    A = Ag.n_agents
+    idx = np.sort(np.random.default_rng(0).choice(A, size=min(A, DUMP_AGENTS), replace=False))
+    idx_dev = torch.as_tensor(idx, device=Ag._s["pos"].device)
+    arrays = {"agent_index": idx.astype(np.float64)}
+    for name in ("pos", "velocity", "rotational_velocity", "measured_velocity", "measured_rotational_velocity",
+                 "head_direction", "distance_travelled", "distance_to_closest_wall"):
+        arrays[f"agent_{name}"] = Ag._s[name][idx_dev].cpu().numpy().astype(np.float64)
+    for k, ns in enumerate(pops):
+        arrays[f"pop{k}_rates"] = ns._hist[ns._last_slot][idx_dev, : ns.n].cpu().numpy().astype(np.float32)
+        if ns.save_history and ns.save_spikes:
+            words = ns._spk[ns._last_slot][idx_dev].cpu().numpy().view(np.uint32)
+            # bit L of word 4B+i = cell 128B + 4L + i (the layout Neurons.get_history_arrays unpacks)
+            bits = np.unpackbits(words.view(np.uint8), axis=-1, bitorder="little")
+            bits = bits.reshape(len(idx), -1, 4, 32).transpose(0, 1, 3, 2).reshape(len(idx), -1)
+            arrays[f"pop{k}_spikes"] = bits[:, : ns.n].astype(np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_BYTES_MAX, f"--dump-outputs would write {total} bytes"
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def measure(rb, lib, torch, dist, name, steps, warmup, rank, world, local_rank, spikes=True, total_agents=None, e2e=True,
-            keep=False):
+            keep=False, dump_dir=None):
     """Device-resident throughput (riab_run, CUDA events, max over ranks) and the stepped-API e2e number of one workload.
-    total_agents: strong-scaling variant (that many agents in total, split over the ranks)."""
+    total_agents: strong-scaling variant (that many agents in total, split over the ranks).
+    dump_dir: write the last timed step's outputs there (dump_outputs), on rank 0, before anything else steps the agents."""
     wl = WORKLOADS[name]
     if total_agents is not None:
         A, scaling = total_agents // world, "strong"
@@ -318,6 +349,8 @@ def measure(rb, lib, torch, dist, name, steps, warmup, rank, world, local_rank, 
     barrier()
     launches = lib.riab_launch_count() - l0
     ms = max_over_ranks(ev0.elapsed_time(ev1))
+    if dump_dir is not None and rank == 0:
+        dump_outputs(torch, Ag, pops, dump_dir)
     res = {"agents_per_gpu": A, "agents_total": A * world, "n_cells": n_cells, "scaling": scaling, "steps": steps,
            "ms_per_step": ms / steps, "value": world * A * steps / (ms * 1e-3), "gpu_launches": int(launches)}
     bytes_unit = algorithmic_bytes_per_agent_step(n_cells, spikes)
@@ -440,6 +473,8 @@ def main():
     ap.add_argument("--no-extra", action="store_true", help="skip the `workloads` / `strong` / `gather` objects")
     ap.add_argument("--agents", type=int, default=None,
                     help="experiments only: agents per GPU instead of the workload's (the line's config says so)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (a fixed sample of agents) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.agents is not None:                          # experiment: same workload at another batch size
         w0 = WORKLOADS[args.workload]
@@ -483,16 +518,17 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     head = measure(rb, lib, torch, dist, args.workload, args.steps, args.warmup, rank, world, local_rank, spikes=spikes,
-                   keep=(world > 1 and not args.no_extra))
+                   keep=(world > 1 and not args.no_extra), dump_dir=args.dump_outputs)
     clocks = sampler.stop()        # sampled across the device-resident and the e2e timed regions of the headline workload
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json (measured)" if peaks else "fallback 6650 GB/s"
-    sm_mhz = clocks.get("sm_mhz") or 1965.0
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json (measured)" if peaks else "H100 SXM data sheet, 3350 GB/s"
+    sm_mhz = clocks.get("sm_mhz") or 1980.0            # (fallback: the H100 SXM's maximum SM clock)
+    n_sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
 
     def roofline_of(name, r):
         rf = {"bound": "hbm", "achieved": r["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": r["achieved_gbs"] / peak,
@@ -500,19 +536,11 @@ def main():
               "kernel_ms": r["ms_per_step"]}
         if "ex2_per_step" in r:
             # BoundaryVectorCells are bound by the special-function unit, not by HBM: one ex2 per (agent, cell, test angle)
-            # in the angular integral (T = 180) against 16 MUFU results per clock per SM (148 SMs at the sampled SM clock)
+            # in the angular integral (T = 180) against 16 MUFU results per clock per SM (every SM at the sampled SM clock)
             ex2 = r["ex2_per_step"] / (r["ms_per_step"] * 1e-3)
-            peak_ex2 = 148 * 16 * sm_mhz * 1e6
+            peak_ex2 = n_sms * 16 * sm_mhz * 1e6
             rf["mufu"] = {"achieved_ex2_per_s": ex2, "peak_ex2_per_s": peak_ex2, "frac": ex2 / peak_ex2,
                           "note": "share of the whole step (motion, rays, other populations included) spent at the ex2 rate"}
-        prof = os.path.join(ROOT, "profiles", f"traffic_{name}.json")
-        if os.path.exists(prof):
-            try:
-                t = json.load(open(prof))
-                rf["traffic"] = t.get("dram_bytes_per_step")
-                rf["traffic_source"] = t.get("source")
-            except Exception:
-                pass
         return rf
 
     extra = {}

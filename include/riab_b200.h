@@ -1,4 +1,4 @@
-/* riab_b200.h -- C ABI of the B200-native batched step engine for RatInABox's
+/* riab_b200.h -- C ABI of the H100-native batched step engine for RatInABox's
  * per-step hot path (Agent.update + Neurons.update for PlaceCells, GridCells,
  * BoundaryVectorCells).
  *

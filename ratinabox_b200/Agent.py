@@ -89,7 +89,7 @@ class Agent:
         #                      (riab_step_fused, one kernel per (motion, cell type));
         #              False = update() launches the motion kernel at once and Neurons.update() the rate kernel: the float64
         #                      motion chain then overlaps the host side of Neurons.update() instead of gating the rate warps
-        #                      inside one kernel (measured faster end to end, profiles/r02_summary.md), and reading
+        #                      inside one kernel (measured faster end to end), and reading
         #                      positions only waits for the motion kernel.
         "fused_step": False,
     }

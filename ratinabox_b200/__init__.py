@@ -1,4 +1,4 @@
-"""ratinabox_b200 -- B200-native batched step engine behind RatInABox's
+"""ratinabox_b200 -- H100-native batched step engine behind RatInABox's
 Environment / Agent / Neurons API (hot path only; see DESIGN.md).
 
     from ratinabox_b200 import Environment, Agent, PlaceCells, GridCells, BoundaryVectorCells

@@ -1,4 +1,4 @@
-"""Build libriab_b200.so in-tree with nvcc for sm_100a (no torch extension machinery:
+"""Build libriab_b200.so in-tree with nvcc for sm_90a (no torch extension machinery:
 the library has a plain C ABI and is loaded with ctypes)."""
 import os
 import subprocess
@@ -11,7 +11,7 @@ SOURCES = ["riab_b200.cu"]
 HEADERS = None  # every csrc/*.cuh + include/riab_b200.h (see _headers)
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr", "-split-compile", "0",
 ]
 

@@ -1,5 +1,5 @@
 // Shared device helpers: non-contracting float64 wrapper, Philox4x32-10, TMA bulk
-// copy + mbarrier primitives (sm_100a), cache-hinted stores.
+// copy + mbarrier primitives (sm_90a), cache-hinted stores.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -161,25 +161,6 @@ RIAB_DEV float ex2f(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-// Packed float32 pairs (PTX f32x2, SASS FFMA2 / FMUL2 / FADD2, sm_100): one issue slot for two FMA-pipe operations on an
-// even-aligned register pair.  `bc2(x)` is the broadcast pair (x, x): ptxas folds it into the instruction's scalar
-// `.F32` operand form, so per-agent shared-memory broadcasts need no duplicated record fields and no MOVs.
-// scripts/ubench_packed.cu: 2.0 cycles per packed instruction per sub-partition = the FMA-pipe time of two scalar
-// operations in one issue slot (the rate consumers are issue-bound, not FMA-pipe bound).
-typedef unsigned long long f32x2;
-RIAB_DEV f32x2 pk2(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-RIAB_DEV f32x2 bc2(float x) { return pk2(x, x); }
-RIAB_DEV void upk2(f32x2 r, float& lo, float& hi) { asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(r)); }
-#ifndef RIAB_SCALAR_PAIRS
-RIAB_DEV f32x2 ffma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-RIAB_DEV f32x2 fmul2(f32x2 a, f32x2 b) { f32x2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-RIAB_DEV f32x2 fadd2(f32x2 a, f32x2 b) { f32x2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-#else   // experiment: the same arithmetic as two scalar FMA-pipe instructions per pair
-RIAB_DEV f32x2 ffma2(f32x2 a, f32x2 b, f32x2 c) { float a0, a1, b0, b1, c0, c1; upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1); return pk2(fmaf(a0, b0, c0), fmaf(a1, b1, c1)); }
-RIAB_DEV f32x2 fmul2(f32x2 a, f32x2 b) { float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1); return pk2(a0 * b0, a1 * b1); }
-RIAB_DEV f32x2 fadd2(f32x2 a, f32x2 b) { float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1); return pk2(a0 + b0, a1 + b1); }
-#endif
 
 // 2^x for x <= 0 on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f through the 1.5*2^23 trick,
 // degree-5 polynomial for 2^f on [-0.5, 0.5] (max relative error 2.5e-7, ex2.approx's own is ~2e-7), exponent

@@ -42,16 +42,14 @@ RIAB_DEV void grid_load_cells(GridCellRegs<CPT>& r, const GridConst& c, int cell
 template <int CPT>
 RIAB_DEV void grid_rates4(float (&out)[CPT], const GridCellRegs<CPT>& r, const GridConst& c, const float* __restrict__ rec) {
   const float2 p = *reinterpret_cast<const float2*>(rec);
-  const f32x2 npx = bc2(-p.x), npy = bc2(-p.y);
+  const float npx = -p.x, npy = -p.y;
 #pragma unroll
-  for (int h = 0; h < CPT / 2; ++h) {                 // cell pairs: the three phases are 2 FFMA2 each per two rates
+  for (int h = 0; h < CPT / 2; ++h) {                 // cell pairs: the three phases are 2 FFMA each per rate
     float s0 = 0.f, s1 = 0.f;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-      f32x2 phi = ffma2(pk2(r.kx[k][2 * h], r.kx[k][2 * h + 1]), npx, pk2(r.ph[k][2 * h], r.ph[k][2 * h + 1]));
-      phi = ffma2(pk2(r.ky[k][2 * h], r.ky[k][2 * h + 1]), npy, phi);
-      float a, b;
-      upk2(phi, a, b);
+      const float a = fmaf(r.ky[k][2 * h], npy, fmaf(r.kx[k][2 * h], npx, r.ph[k][2 * h]));
+      const float b = fmaf(r.ky[k][2 * h + 1], npy, fmaf(r.kx[k][2 * h + 1], npx, r.ph[k][2 * h + 1]));
       if (k == 0) { s0 = __cosf(a); s1 = __cosf(b); }
       else { s0 += __cosf(a); s1 += __cosf(b); }
     }

@@ -15,7 +15,7 @@
 // 0<l_a<1 and 0<l_b<1.  With f = signed distance to the wall's line and t = the
 // parameter along the wall, l_a = f_c/(f_c-f_p) and l_b = (f_c t_p - f_p t_c)/(f_c-f_p),
 // so per (agent, cell, wall) the float32 fast path is three scalar FMA-pipe operations on
-// per-cell registers and per-agent shared-memory broadcasts and one three-input FMNMX3; the
+// per-cell registers and per-agent shared-memory broadcasts and a three-way min; the
 // select is arithmetic (the penalty enters the exponent).  Results within an absolute
 // band of 0 are re-evaluated in float64 with the reference's exact expression
 // (los_blocked_exact), so the decision equals the oracle's.
@@ -227,10 +227,10 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
     // Everything is divided by b on the agent side and carries -sign(f_p) (record: -s t_p/b, -s (1-t_p)/b, band/b), so
     //   X = M'/b = fma(f_c, -s t_p/b, t_c),  Y = (|D|-M')/b = fma(f_c, -s (1-t_p)/b, 1-t_c),  q' = f_c (-f_p 2^20)
     // hold whenever q' > 0 (f_c * -s = a then); on the same side q' < 0 decides alone.  m3 = min(X, Y, q'):
-    // per cell 2 FFMA + 1 FMUL (agent values from the record) + 1 FMNMX3;
+    // per cell 2 FFMA + 1 FMUL (agent values from the record) + 2 FMNMX;
     // blocked <=> m3 > 0.
     // |m3| below band/b => the sign of m3 is not certain in float32: re-evaluate in float64.
-    // The select is arithmetic: pen = max(0, max_j m3_j) (one FMNMX3 for two walls; NaN -> 0) enters the exponent /
+    // The select is arithmetic: pen = max(0, max_j m3_j) (NaN -> 0) enters the exponent /
     // the squared distance multiplied by 2^100: any pen above the band (>= ~1e-6 / b) makes the rate exactly 0.
     float worst[CPT], m3_prev[CPT];                       // worst = max(0, max over walls of m3)
 #pragma unroll
@@ -242,8 +242,6 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
       float m3[CPT];
 #pragma unroll
       for (int i = 0; i < CPT; ++i) {
-        // scalar FMA-pipe operations: packed FFMA2 / FMUL2 here measured SLOWER in this mix with FMNMX3 (16.2 vs 13.1 cycles
-        // per cell pair and wall, scripts/ubench_packed.cu: a packed instruction holds the math dispatch port two cycles)
         const float fc = r.fc[j][i];
         const float X = fmaf(fc, pw.x, r.tc[j][i]);
         const float Y = fmaf(fc, pw.y, r.tq[j][i]);
@@ -251,7 +249,7 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
       }
 #pragma unroll
       for (int i = 0; i < CPT; ++i) {
-        if ((j & 1) == 1) worst[i] = fmaxf(fmaxf(worst[i], m3[i]), m3_prev[i]);   // pairs of walls: one FMNMX3
+        if ((j & 1) == 1) worst[i] = fmaxf(fmaxf(worst[i], m3[i]), m3_prev[i]);   // pairs of walls
         else if (j == WI - 1) worst[i] = fmaxf(worst[i], m3[i]);                                    // odd wall count: the last one
         m3_prev[i] = m3[i];
       }
@@ -273,15 +271,11 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
   // 1 FADD + 2 FFMA per rate on per-cell registers (2k cx, 2k cy, -k|c|^2); only used when k * r2_max <= 10,
   // where the cancellation costs < 4e-6 relative (make_place).  Blocked pairs: exponent - 1e5 -> rate 0 (d = 1000).
   if (DESC == RIAB_PC_GAUSSIAN && (EXP >= 1 || (EXP < 0 && c.expanded))) {
-    const f32x2 zz = bc2(r0.z), px2 = bc2(r0.x), py2 = bc2(r0.y);
 #pragma unroll
-    for (int h = 0; h < CPT / 2; ++h) {                   // cell pairs: FADD2 + 2 (3) FFMA2 per two rates
-      f32x2 t = fadd2(pk2(r.k[2 * h], r.k[2 * h + 1]), zz);
-      t = ffma2(pk2(r.cx[2 * h], r.cx[2 * h + 1]), px2, t);
-      t = ffma2(pk2(r.cy[2 * h], r.cy[2 * h + 1]), py2, t);
-      if (WI > 0) t = ffma2(pk2(pen[2 * h], pen[2 * h + 1]), bc2(-PLACE_PEN), t);
-      float t0, t1;
-      upk2(t, t0, t1);
+    for (int h = 0; h < CPT / 2; ++h) {                   // cell pairs: FADD + 2 (3) FFMA per rate
+      float t0 = fmaf(r.cy[2 * h], r0.y, fmaf(r.cx[2 * h], r0.x, r.k[2 * h] + r0.z));
+      float t1 = fmaf(r.cy[2 * h + 1], r0.y, fmaf(r.cx[2 * h + 1], r0.x, r.k[2 * h + 1] + r0.z));
+      if (WI > 0) { t0 = fmaf(pen[2 * h], -PLACE_PEN, t0); t1 = fmaf(pen[2 * h + 1], -PLACE_PEN, t1); }
       // Neurons.py:978-980; EXP == 2: min_fr == 0 and log2(span) already sits in the agent's -k|p|^2 term
       if (EXP == 2 || (EXP < 0 && c.fold)) { out[2 * h] = ex2f(t0); out[2 * h + 1] = ex2f(t1); }
       else { out[2 * h] = fmaf(ex2f(t0), c.span, c.min_fr); out[2 * h + 1] = fmaf(ex2f(t1), c.span, c.min_fr); }
