@@ -245,7 +245,8 @@ int riab_ovc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, co
  * rates already written to rates_dev.  noise_dev (A,N) f32 state (NULL when
  * noise_std == 0); spikes (A, 4*ceil(N/128)) uint32 words (layout: riab_rates_out.spikes_row), NULL to skip. */
 typedef struct {
-  float noise_std, noise_coherence_time, dt;
+  float noise_std, noise_coherence_time;
+  double dt;                /* the Agent's dt: the thinned spike stream's tables and the OU constants use it in float64 */
   uint64_t seed, step;
   int64_t id_offset;
   int32_t population_id;    /* distinguishes the Philox streams of populations of one Agent */

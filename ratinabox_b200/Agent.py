@@ -468,10 +468,14 @@ class Agent:
         _lib.check(self._lib.riab_run(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
                                       C.byref(self._io), pops, len(self.Neurons), C.byref(hist), n_steps,
                                       self._stream()))
-        # host-side bookkeeping of the n_steps that just ran
-        t0 = self.t - dt
-        ts = [t0 + dt * (k + 1) for k in range(n_steps)]
-        self.prev_t, self.t = ts[-2] if n_steps > 1 else t0, ts[-1]
+        # host-side bookkeeping of the n_steps that just ran: the clock advances by `t += dt` per step like update()
+        # (the staging update() above already made the first), so the times equal the stepped loop's bit for bit
+        ts = [self.t]
+        for _ in range(n_steps - 1):
+            ts.append(ts[-1] + dt)
+        if n_steps > 1:
+            self.prev_t = ts[-2]
+        self.t = ts[-1]
         self._step = first_step + n_steps
         if self.save_history:
             self._hist_rows += n_steps

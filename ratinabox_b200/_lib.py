@@ -80,7 +80,7 @@ class HistoryView(C.Structure):
 
 
 class NeuronNoise(C.Structure):
-    _fields_ = [("noise_std", C.c_float), ("noise_coherence_time", C.c_float), ("dt", C.c_float),
+    _fields_ = [("noise_std", C.c_float), ("noise_coherence_time", C.c_float), ("dt", C.c_double),
                 ("seed", C.c_uint64), ("step", C.c_uint64), ("id_offset", C.c_int64), ("population_id", C.c_int32)]
 
 

@@ -941,6 +941,9 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
       // tile, so a tile's steps are ordered -- and publishes each (step, tile) record into its private ring (slots
       // pw + MW * i): the n-th record it produces goes to slot i = n % NSP in phase n / NSP
       constexpr int NSP = NS / MW;
+      // its clear of a tile's spike rows for step s+1 may overlap the ORs of up to NSP - 1 earlier steps of that tile, so
+      // those steps must have other rows: riab_run launches whole runs with spikes only for ring_rows >= 2 >= NSP
+      static_assert(NSP <= 2, "riab_run launches whole runs with spike rings of 2 rows");
       const long long npw = (nq > pw) ? (nq - pw + MW - 1) / MW : 0;
       long long n = 0;
       for (long long st = 0; st < run.n_steps; ++st) {
@@ -2270,7 +2273,7 @@ static int neurons_update_impl(const riab_agents* agents, const riab_env* env, c
   riab_step_io io0; memset(&io0, 0, sizeof(io0));
   const riab_motion_params& mp = (MODE != 0) ? *prm : mp0;
   const riab_step_io& sio = (MODE != 0) ? *io : io0;
-  const double dt = (prm != nullptr) ? prm->dt : (noise ? (double)noise->dt : 1.0);
+  const double dt = (prm != nullptr) ? prm->dt : (noise ? noise->dt : 1.0);
   const double* pos_in = (MODE == 1) ? nullptr : agents->pos;
   cudaStream_t s = (cudaStream_t)stream;
   if (cells_kind == RIAB_CELLS_PLACE) {
@@ -2350,7 +2353,11 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
   int rc;
   // ---- a single Place / Grid population: the whole run as ONE launch (k_step MODE 3, see RunK) where the lean consumer
   // loop applies: vector-aligned rows, whole 4-cell groups, all cells in one register set, consumer groups that divide the
-  // producers, no OU noise, no parity taps, and rings that hold the run without wrapping onto rows still being written
+  // producers, no OU noise, no parity taps, and no spike ring of a single row.  Rings of any depth may wrap: a tile's rows
+  // of step s are written by one consumer group in step order.  But a producer clears its tile's spike rows of step s+1 as
+  // soon as its private ring (at most 2 records) has room, while the consumers may still RED.OR step s's thinned spikes;
+  // with ring_rows >= 2 those are different rows, with one row nothing orders the clear after the ORs, so that case takes
+  // the per-step loop (stream-ordered launches)
   if (n_pops == 1 && skew && getenv("RIAB_NO_WHOLE_RUN") == nullptr && io->drift_velocity == nullptr && io->pos_mirror == nullptr) {
     const riab_population& pp = pops[0];
     EnvK ek;
@@ -2377,7 +2384,7 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
       ro.rates_row = pp.rates_ring;                                    // (alignment / vector checks of make_out)
       ro.spikes_row = pp.spikes_ring;
       riab_neuron_noise nz = pp.noise;
-      nz.dt = (float)prm->dt;
+      nz.dt = prm->dt;
       if ((rc = make_out(&ro, &nz, n_cells, prm->dt, agents->id_offset, ok, bound))) return rc;
       const int ct = n_pad / 4;
       const bool rows_ok = ((A * ok.ld) % 4 == 0) && ((A * ok.spike_ld) % 4 == 0);        // every ring row stays 16-byte aligned
@@ -2385,7 +2392,8 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
                         (ok.spikes == nullptr || (agents->id_offset & 1) == 0) &&
                         (4 % lean_groups(ct, 8) == 0) && (4 % lean_groups(ct, 4) == 0);      // groups divide the 4 producers
       const bool hist_ok = hist == nullptr || hist->ring == nullptr || hist->ring_rows > 0;
-      if (lean && hist_ok) {
+      const bool spike_ring_ok = pp.spikes_ring == nullptr || pp.ring_rows >= 2;
+      if (lean && hist_ok && spike_ring_ok) {
         RunK run;
         memset(&run, 0, sizeof(run));
         run.n_steps = n_steps;
@@ -2482,7 +2490,7 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
       ro.spikes_row = pp.spikes_ring ? pp.spikes_ring + slot * A * (size_t)(4 * ((n_cells + 127) / 128)) : nullptr;
       riab_neuron_noise nz = pp.noise;
       nz.step = pp.noise.step + (uint64_t)st;
-      nz.dt = (float)prm->dt;
+      nz.dt = prm->dt;
       if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
       else if (p == 0 && st + 1 < n_steps) {
         const riab_step_io nxt = step_io(st + 1);          // the motion it runs belongs to step st+1

@@ -372,6 +372,37 @@ def test_history_rate_maps_on_the_device():
     assert Ag.get_position_heatmap().shape == (20, 20)
 
 
+def test_history_rate_maps_after_the_rings_wrapped():
+    """The same maps after the Agent ring (30 rows) and the population rings (17 and 23 rows) all wrapped inside one
+    Ag.run: the heat-map bins the Agent's last 30 rows, each rate map the last min(30, population rows) rows of both
+    rings -- equal to utils.bin_data_for_histogramming of the host get_history_arrays() of those steps."""
+    import ratinabox_b200 as rb
+    A, pre, steps = 300, 3, 40
+    E, Ag = make(rb, A, dt=0.05, history_bytes_limit=30 * A * 32)
+    PCs = rb.PlaceCells(Ag, {"n": 20, "widths": 0.3, "history_bytes_limit": 17 * A * 20 * 4})
+    GCs = rb.GridCells(Ag, {"n": 6, "history_bytes_limit": 23 * A * 8 * 4})
+    for _ in range(pre):
+        Ag.update(); PCs.update(); GCs.update()
+    Ag.run(steps)
+    hp = Ag.get_history_arrays()["pos"]
+    assert hp.shape == (30, A, 2) and Ag.history_dropped == pre + steps - 30
+    dx = 0.1
+    heat = Ag.get_position_heatmap(dx=dx)
+    ref = O.bin_data_for_histogramming(hp.reshape(-1, 2), list(E.extent), dx)
+    assert np.array_equal(heat, ref) and heat.sum() == 30 * A
+    for Ns, rows in ((PCs, 17), (GCs, 23)):
+        h = Ns.get_history_arrays()
+        assert h["firingrate"].shape == (rows, A, Ns.n) and Ns.history_dropped == pre + steps - rows
+        pos = hp[-rows:].reshape(-1, 2)
+        fr = h["firingrate"].reshape(-1, Ns.n)
+        maps, zero = Ns.get_history_rate_maps(dx=dx, return_zero_bins=True)
+        for c in range(Ns.n):
+            m, zb = O.bin_data_for_histogramming(pos, list(E.extent), dx, weights=fr[:, c], norm_by_bincount=True,
+                                                 return_zero_bins=True)
+            assert np.array_equal(zero, zb)
+            assert np.abs(maps[c] - m).max() <= 1e-5 * max(1.0, np.abs(m).max())
+
+
 def test_step_fused_host_entry_point():
     """riab_step_fused_host (the C-ABI e2e entry: HOST drift in, fused step, HOST positions out) equals the Python
     API's own step bit for bit."""

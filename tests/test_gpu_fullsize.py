@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 import riab_oracle as O
-from philox_np import agent_normals
+from philox_np import agent_normals, expected_spikes_of
 
 pytestmark = pytest.mark.gpu
 
@@ -98,6 +98,60 @@ def test_config3_65536_agents_1024_grid_cells():
     env, ref_pos = _oracle_positions([], pos0, vel0, sample, steps)
     assert np.abs(pos[sample] - ref_pos).max() <= 1e-6
     ref = O.grid_cells_get_state(GCs.gridscales, GCs.phase_offsets, GCs.w, pos[sample]).T
+    assert np.abs(fr[sample] - ref).max() <= 1e-5
+    # the whole run's thinned spike stream (dt * max_fr = 0.01): the last row bit for bit against the NumPy mirror
+    h = GCs.get_history_arrays()
+    assert np.array_equal(h["firingrate"][-1], fr)
+    want = expected_spikes_of(GCs, 5, steps - 1, sample, fr[sample], 0.01, fr_bound=1.0)
+    assert np.array_equal(h["spikes"][-1][sample], want)
+    assert want.any()
+
+
+def _ring_spikes(ns, slot, agents):
+    """Spike bits of ring row `slot` for some agents (get_history_arrays' unpacking: bit L of word 4B+i = cell 128B+4L+i)."""
+    import torch
+    words = ns._spk[slot][torch.as_tensor(agents, device=ns._spk.device)].cpu().numpy().view(np.uint32)
+    bits = np.unpackbits(words.view(np.uint8), axis=-1, bitorder="little")
+    return bits.reshape(len(agents), -1, 4, 32).transpose(0, 1, 3, 2).reshape(len(agents), -1)[:, : ns.n].astype(bool)
+
+
+def test_config3_whole_run_wraps_the_default_ring():
+    """configs[2]'s population at full size, 40 steps of Ag.run after 3 stepped ones: a 65 536 x 1 024 rate row is 256 MiB,
+    so the default 8 GiB history_bytes_limit holds 32 rows and the whole run (one launch) wraps its rings in the middle.
+    The last row is the step's output and the last two retained rows carry the thinned spikes of their steps."""
+    import torch
+    import ratinabox_b200 as rb
+    from ratinabox_b200 import _lib
+    lib = _lib.load()
+    A, N, pre, steps = 65536, 1024, 3, 40
+    E, Ag = _setup(rb, A, [])
+    pos0, vel0 = Ag.pos.copy(), Ag.velocity.copy()
+    rs = np.random.RandomState(3)
+    GCs = rb.GridCells(Ag, {"gridscale": rs.uniform(0.2, 1.0, N), "orientation": rs.uniform(0, np.pi / 3, N),
+                            "phase_offset": rs.uniform(0, 2 * np.pi, (N, 2))})
+    for _ in range(pre):
+        Ag.update(); GCs.update()
+    c0 = lib.riab_launch_count()
+    Ag.run(steps)
+    assert lib.riab_launch_count() - c0 == 1                 # k_step MODE 3
+    total = pre + steps
+    cap = GCs._hist_cap
+    assert cap == (8 << 30) // (A * N * 4) == 32 and GCs._hist_rows == total
+    ha = Ag.get_history_arrays()
+    assert Ag.history_dropped == 0 and ha["pos"].shape == (total, A, 2)
+    last = (total - 1) % cap
+    fr = GCs.firingrate
+    assert np.array_equal(GCs._hist[last][:, :N].cpu().numpy().astype(np.float64), fr)
+    sample = np.random.RandomState(6).choice(A, 256, replace=False)
+    for k in (1, 2):
+        slot = (total - k) % cap
+        rates = GCs._hist[slot][torch.as_tensor(sample, device=GCs._hist.device), :N].cpu().numpy()
+        want = expected_spikes_of(GCs, 5, total - k, sample, rates, 0.01, fr_bound=1.0)
+        assert np.array_equal(_ring_spikes(GCs, slot, sample), want), k
+    torch.cuda.synchronize()
+    env, ref_pos = _oracle_positions([], pos0, vel0, sample[:64], total)
+    assert np.abs(Ag.pos[sample[:64]] - ref_pos).max() <= 1e-6
+    ref = O.grid_cells_get_state(GCs.gridscales, GCs.phase_offsets, GCs.w, Ag.pos[sample]).T
     assert np.abs(fr[sample] - ref).max() <= 1e-5
 
 
