@@ -48,10 +48,6 @@ constexpr int TA = 32;      // agents per tile (one warp runs their motion)
 constexpr int NT = 256;     // threads per CTA in the tile kernels
 constexpr int MAXW = 64;    // walls staged in shared memory
 constexpr int CELL_PAD = 128;  // packed per-cell arrays are padded to 4 cells x 32 lanes
-#ifndef RIAB_BVC_MUFU_TERMS
-#define RIAB_BVC_MUFU_TERMS 8
-#endif
-constexpr int BVC_MUFU_TERMS = RIAB_BVC_MUFU_TERMS;   // of 8 agents per thread: exponentials on the MUFU pipe (rest: ex2_fma)
 
 struct EnvK {
   const double* walls;
@@ -172,19 +168,12 @@ struct RowCursor {
   unsigned long long gid;  // global agent id
 };
 
-template <int CPT = 4>
-__device__ __forceinline__ void tail_init(TailCtx& t, const OutK& out, int cell0, int n_cells, unsigned long long step);
-template <int CPT = 4>
-__device__ __forceinline__ void tail_init(TailCtx& t, const OutK& out, int cell0, int n_cells) {
-  tail_init<CPT>(t, out, cell0, n_cells, out.step);
-}
-template <int CPT>
 __device__ __forceinline__ void tail_init(TailCtx& t, const OutK& out, int cell0, int n_cells, unsigned long long step) {
   t.cell0 = cell0; t.n_cells = n_cells;
   t.vmask = 0u;
 #pragma unroll
-  for (int i = 0; i < CPT; ++i) t.vmask |= (cell0 + i < n_cells) ? (1u << i) : 0u;
-  t.full4 = out.vec_ok && (t.vmask == ((1u << CPT) - 1u));
+  for (int i = 0; i < 4; ++i) t.vmask |= (cell0 + i < n_cells) ? (1u << i) : 0u;
+  t.full4 = out.vec_ok && (t.vmask == 0xfu);
   t.sub = (uint32_t)(cell0 >> 2);
   t.c2 = (uint32_t)step;
   const uint32_t hi = ((uint32_t)(step >> 32) & 0xffffu) | (((uint32_t)out.pop & 0xffu) << 16);
@@ -269,21 +258,12 @@ __device__ __forceinline__ float spike_neg_dither(const uint32_t (&c)[4]) {
   return (float)((c[0] ^ c[2]) >> 8) * -5.9604644775390625e-08f;
 }
 // ballots of one agent's 4 cell slots; `ok` = this thread's cells exist (all 4 or none) when !MASKED.
-// XU_BOUND: for a cell type that saturates the XU pipe the four integer -> float conversions can be done as
-// as_float(0x4B000000 | m) - 2^23  (PRMT + FADD, exact, same bits) instead of I2F; no current policy needs it.
-template <bool MASKED, bool XU_BOUND = false>
+template <bool MASKED>
 __device__ __forceinline__ void spike_ballots(uint32_t (&b)[4], uint32_t w0, uint32_t w1, float nv, const float (&o)[4],
                                               float q /* dt * 65536 */, unsigned vmask, bool ok) {
-  float m0, m1, m2, m3;           // the four 16-bit integers as floats
-  if (XU_BOUND) {
-    m0 = __uint_as_float(__byte_perm(w0, 0x4B000000u, 0x7610)) - 8388608.0f;
-    m1 = __uint_as_float(__byte_perm(w0, 0x4B000000u, 0x7632)) - 8388608.0f;
-    m2 = __uint_as_float(__byte_perm(w1, 0x4B000000u, 0x7610)) - 8388608.0f;
-    m3 = __uint_as_float(__byte_perm(w1, 0x4B000000u, 0x7632)) - 8388608.0f;
-  } else {                        // I2F.U16 reads either half-word directly
-    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f32.u16 %0, l;\n\tcvt.rn.f32.u16 %1, h;\n\t}" : "=f"(m0), "=f"(m1) : "r"(w0));
-    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f32.u16 %0, l;\n\tcvt.rn.f32.u16 %1, h;\n\t}" : "=f"(m2), "=f"(m3) : "r"(w1));
-  }
+  float m0, m1, m2, m3;           // the four 16-bit integers as floats (I2F.U16 reads either half-word directly)
+  asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f32.u16 %0, l;\n\tcvt.rn.f32.u16 %1, h;\n\t}" : "=f"(m0), "=f"(m1) : "r"(w0));
+  asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f32.u16 %0, l;\n\tcvt.rn.f32.u16 %1, h;\n\t}" : "=f"(m2), "=f"(m3) : "r"(w1));
   bool s0 = m0 < fmaf(o[0], q, nv);
   bool s1 = m1 < fmaf(o[1], q, nv);
   bool s2 = m2 < fmaf(o[2], q, nv);
@@ -312,6 +292,27 @@ __device__ __forceinline__ void spikes1(const float (&o)[4], const OutK& out, co
   spike_ballots<true>(b, h ? c[2] : c[0], h ? c[3] : c[1], nv, o, out.dt * 65536.0f, t.vmask, true);
   spike_store(b, rc.spk);
 }
+// agents rc.gid and, if has_b, rc.gid + 1 of the general path (whole warp must call): one Philox call for a complete pair
+// that starts on an even id, else one per agent
+__device__ __forceinline__ void spikes_pair(const float (&oa)[4], const float (&ob)[4], const bool has_b, const bool even,
+                                            const OutK& out, const TailCtx& t, const RowCursor& rc, const float q16) {
+  if (has_b && even) {
+    uint32_t c[4], bl[4];
+    spike_words(c, out, t, rc.gid);
+    const float nv = spike_neg_dither(c);
+    spike_ballots<true>(bl, c[0], c[1], nv, oa, q16, t.vmask, true);
+    spike_store(bl, rc.spk);
+    spike_ballots<true>(bl, c[2], c[3], nv, ob, q16, t.vmask, true);
+    spike_store(bl, rc.spk + out.spike_ld);
+  } else {
+    spikes1(oa, out, t, rc);
+    if (has_b) {
+      RowCursor rb = rc;
+      rb.gid += 1; rb.spk += out.spike_ld;
+      spikes1(ob, out, t, rb);
+    }
+  }
+}
 
 template <bool SPIKES, bool NOISE>
 __device__ __forceinline__ void finish4(float (&o)[4], const OutK& out, const TailCtx& t, const RowCursor& rc) {
@@ -321,14 +322,12 @@ __device__ __forceinline__ void finish4(float (&o)[4], const OutK& out, const Ta
 
 // ---------------------------------------------------------------------------
 // Cell-type policies for the step kernel.
-template <int WI, int DESC, int CPT_ = 4>
+template <int WI, int DESC>
 struct PlacePolicy {
   using Const = PlaceConst;
-  using Regs = PlaceCellRegs<WI, CPT_>;
-  static constexpr int CPT = CPT_;                          // cells per consumer thread
+  using Regs = PlaceCellRegs<WI>;
   static constexpr int REC = place_rec(WI);
   static constexpr bool LIGHT = (WI == 0) && (DESC >= 0);   // few instructions per rate: HBM-bound consumers
-  static constexpr bool XU_BOUND = false;
   // rates lie in [min_fr, max_fr], so the thinned spike stream applies, but it measured slower for place cells: the
   // Euclidean Gaussian loop is HBM-bound and hides the dense stream's instructions under its stores, the line-of-sight
   // loop with the post-pass needs 8 producer warps and loses next to them.  The dense stream stays.
@@ -341,26 +340,23 @@ struct PlacePolicy {
                                                 const double* aux, const Const& c, const EnvK& env) {
     place_agent_record<WI>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
   }
-  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI, CPT_>(r, c, cell0); }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI>(r, c, cell0); }
   template <bool DEFER, int EXP = -1>
-  static __device__ __forceinline__ void rates4(float (&o)[CPT_], const Regs& r, const Const& c, int cell0,
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int cell0,
                                                 const float* rec, uint32_t inner_s, bool& unsure) {
-    place_rates4<WI, DESC, DEFER, EXP, CPT_>(o, r, c, cell0, rec, inner_s, unsure);
+    place_rates4<WI, DESC, DEFER, EXP>(o, r, c, cell0, rec, inner_s, unsure);
   }
   // 0: direct form, 1: expanded exponent, 2: expanded with the [0, max_fr] scale folded into the exponent
   static __device__ __forceinline__ int expanded(const Const& c) { return (DESC == RIAB_PC_GAUSSIAN && c.expanded) ? 1 + c.fold : 0; }
   static __device__ __forceinline__ int wall0(const Const& c) { return c.wall0; }
 };
 
-template <int CPT_ = 4>
 struct GridPolicy {
   using Const = GridConst;
-  using Regs = GridCellRegs<CPT_>;
-  static constexpr int CPT = CPT_;
+  using Regs = GridCellRegs;
   static constexpr int REC = 4;
   static constexpr bool LIGHT = false;    // 36 cell registers per thread do not fit StepCfg<8>'s 56-register consumers
   static constexpr bool THIN = true;      // bounded rates, consumer-bound loop: thinned spikes
-  static constexpr bool XU_BOUND = false; // 3 MUFU.COS per rate, yet issue-bound: PRMT+FADD instead of I2F measured slower
   static __device__ __forceinline__ const double* head_dir(const Const&) { return nullptr; }
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
   static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, const double*, const double*,
@@ -368,11 +364,11 @@ struct GridPolicy {
     rec[0] = (float)(px - env.cxm);
     rec[1] = (float)(py - env.cym);
   }
-  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { grid_load_cells<CPT_>(r, c, cell0); }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { grid_load_cells(r, c, cell0); }
   template <bool DEFER, int EXP = -1>
-  static __device__ __forceinline__ void rates4(float (&o)[CPT_], const Regs& r, const Const& c, int, const float* rec,
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
                                                 uint32_t, bool&) {
-    grid_rates4<CPT_>(o, r, c, rec);
+    grid_rates4(o, r, c, rec);
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const&) { return 0; }
@@ -381,11 +377,9 @@ struct GridPolicy {
 struct OvcPolicy {
   using Const = OvcConst;
   using Regs = OvcCellRegs;
-  static constexpr int CPT = 4;
   static constexpr int REC = OVC_REC;
   static constexpr bool LIGHT = false;
   static constexpr bool THIN = false;     // sums over objects: no a-priori rate bound
-  static constexpr bool XU_BOUND = false;
   static __device__ __forceinline__ const double* head_dir(const Const& c) { return c.head_dir; }
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
   static __device__ __forceinline__ void record(float* rec, double px, double py, double hdx, double hdy,
@@ -483,50 +477,44 @@ struct __align__(16) StepSlot {
   int pad[2];
 };
 
-// The consumers' hot loop: consecutive agent pairs (2p, 2p+1) of one ring slot, 4 cells per thread, no OU noise,
-// 16-byte aligned rows, even first global id.  The line-of-sight band test is deferred: a pair whose float32 decision fell
-// inside the band only sets its bit in `redo`; the caller redoes those pairs through the general path
-// (per-agent exact float64 fall-back) after the loop -- no call and no branch in here.
-// DENSE: the dense spike stream (one Philox4x32-7 call per pair, a threshold test per rate) runs in the loop;
-// thinned spikes are a post-pass over the slot (thin_block) and leave this loop spike-free.
+// The consumers' hot loop: n2 consecutive agent pairs (2p, 2p+1) of one ring slot, no OU noise, 16-byte aligned rows
+// (ld floats apart), every thread's 4 cells exist or none (`act`).  recp and d (the first agent's record, rate row + cell0)
+// advance past the pairs, with DENSE also spk and pair (spike row + ballot words, global id / 2).  The line-of-sight band
+// test is deferred: a pair whose float32 decision fell inside the band only sets its bit in `redo`; the caller redoes
+// those pairs through the general path (per-agent exact float64 fall-back) after the loop -- no call, no branch in here.
+// DENSE: the dense spike stream (one Philox4x32-7 call per pair, a threshold test per rate; needs an even first global
+// id) runs in the loop; thinned spikes are a post-pass over the slot (thin_block) and leave this loop spike-free.
 template <class P, bool DENSE, int EXP>
-__device__ __forceinline__ void consume_pairs(int& a, const int a_end, const typename P::Regs& regs,
-                                              const typename P::Const& pc, const OutK& out, const TailCtx& tc,
-                                              const int cell0, const float*& recp, const uint32_t inner_s, RowCursor& rc,
-                                              const bool act, const float q16, uint32_t& redo) {
-  float* dst = rc.dst;
-  uint32_t bit = 1u;
-  uint32_t* spk = rc.spk;
-  unsigned long long pair = rc.gid >> 1;
-  const long long pair_rate = 2ll * out.ld, pair_spk = 2ll * out.spike_ld;     // elements per pair step
-  for (; a + 1 < a_end; a += 2) {
-    float o[P::CPT];
+__device__ __forceinline__ void consume_pairs(const int n2, const typename P::Regs& regs, const typename P::Const& pc,
+                                              const OutK& out, const TailCtx& tc, const int cell0, const float*& recp,
+                                              const uint32_t inner_s, const long long ld, float*& d, uint32_t*& spk,
+                                              unsigned long long& pair, const bool act, const float q16, uint32_t& redo) {
+  for (int it = 0; it < n2; ++it) {
+    float o[4];
     uint32_t c[4], bl[4];
     bool unsure = false;
     P::template rates4<true, EXP>(o, regs, pc, cell0, recp, inner_s, unsure);
-    if (act) st_cs_fv<P::CPT>(dst, o);
+    if (act) st_cs_f4(d, o);
     float nv = 0.f;
-    if constexpr (DENSE && P::CPT == 4) {
+    if constexpr (DENSE) {
       c[0] = (uint32_t)pair; c[1] = tc.sub ^ ((uint32_t)(pair >> 32) << 24); c[2] = tc.c2; c[3] = tc.c3_spk;
       philox_keyed<7>(c, out.rk7);
       nv = spike_neg_dither(c);
-      spike_ballots<false, P::XU_BOUND>(bl, c[0], c[1], nv, o, q16, 0u, act);
+      spike_ballots<false>(bl, c[0], c[1], nv, o, q16, 0u, act);
       spike_store(bl, spk);
     }
     P::template rates4<true, EXP>(o, regs, pc, cell0, recp + P::REC, inner_s, unsure);
-    if (act) st_cs_fv<P::CPT>(dst + out.ld, o);
-    if constexpr (DENSE && P::CPT == 4) {
-      spike_ballots<false, P::XU_BOUND>(bl, c[2], c[3], nv, o, q16, 0u, act);
+    if (act) st_cs_f4(d + ld, o);
+    if constexpr (DENSE) {
+      spike_ballots<false>(bl, c[2], c[3], nv, o, q16, 0u, act);
       spike_store(bl, spk + out.spike_ld);
+      spk += 2 * out.spike_ld;
+      pair += 1ull;
     }
-    redo |= unsure ? bit : 0u;
-    bit <<= 1;
-    dst += pair_rate;
-    spk += pair_spk;
-    pair += 1ull;
+    redo |= (unsure ? 1u : 0u) << it;
+    d += 2 * ld;
     recp += 2 * P::REC;
   }
-  rc.dst = dst; rc.spk = spk; rc.gid = pair << 1;
 }
 
 // ---------------------------------------------------------------------------
@@ -616,9 +604,7 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
   constexpr int NS = ring_slots<P, C>();
   constexpr int NC = RW * 32;
   constexpr bool DENSE = (SPK == 1);
-  constexpr int CPT = P::CPT;
-  static_assert(CPT == 4 || (SPK != 1 && !NOISE), "2 cells per thread: no dense spikes / OU noise (ballot layout)");
-  const int CT = pc.n_pad / CPT;                      // cell-threads needed (multiple of 32)
+  const int CT = pc.n_pad / 4;                        // cell-threads needed (multiple of 32)
   const int chunks = (CT + NC - 1) / NC;
   const int G = (chunks == 1) ? (NC / CT) : 1;        // agent groups when the cells need fewer threads
   const int grp = (chunks == 1) ? (ctid / CT) : 0;
@@ -626,11 +612,11 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
   // group `grp` takes the consecutive agents [2 grp PPG, 2 (grp+1) PPG) of a slot (PPG pairs)
   const int PPG = (TA / 2 + G - 1) / G;
   typename P::Regs regs;
-  int cell0 = (chunks == 1) ? (ctid % CT) * CPT : 0;
+  int cell0 = (chunks == 1) ? (ctid % CT) * 4 : 0;
   TailCtx tc;
   if (chunks == 1 && !idle) {
     P::load(regs, pc, cell0);
-    tail_init<CPT>(tc, out, cell0, pc.n_cells);
+    tail_init(tc, out, cell0, pc.n_cells, out.step);
   }
   const uint32_t inner_s = smem_u32(s_walls) + 32u * (uint32_t)P::wall0(pc);   // float64 inner walls (exact fall-back)
   // Fast pair loop: rows are 16-byte aligned and every thread owns 4 existing cells or none, the
@@ -648,10 +634,10 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
     // the cells in chunks of 2048 and reload their registers per chunk (G = 1, all warps on the same agents)
     for (int ch = 0; ch < chunks; ++ch) {
       if (chunks > 1) {
-        cell0 = (ch * NC + ctid) * CPT;
+        cell0 = (ch * NC + ctid) * 4;
         if (cell0 >= pc.n_pad) continue;              // warp-uniform (n_pad is a multiple of 128)
         P::load(regs, pc, cell0);
-        tail_init<CPT>(tc, out, cell0, pc.n_cells);
+        tail_init(tc, out, cell0, pc.n_cells, out.step);
       } else if (idle) {
         continue;
       }
@@ -666,7 +652,11 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
         uint32_t only = 0xffffffffu;       // pairs (by iteration index) the general loop below evaluates
         if (fast) {
           uint32_t redo = 0u;
-          consume_pairs<P, DENSE, EXP>(a, a_hi, regs, pc, out, tc, cell0, recp, inner_s, rc, act, q16, redo);
+          const int n2 = (a_hi - a_lo) >> 1;
+          unsigned long long pair = rc.gid >> 1;
+          consume_pairs<P, DENSE, EXP>(n2, regs, pc, out, tc, cell0, recp, inner_s, out.ld, rc.dst, rc.spk, pair, act, q16, redo);
+          a += 2 * n2;
+          rc.gid = pair << 1;                      // rc.spk / rc.gid advance with DENSE, the only case that reads them below
           redo = __reduce_or_sync(0xffffffffu, redo);
           if (const unsigned nm = s_slot[s].nanmask; nm != 0u)          // pairs with a NaN position: zero rates below
             for (int it = 0; a_lo + 2 * it < a_hi; ++it)
@@ -684,7 +674,7 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
         const RowStride stride = make_stride(out, 2);
         const bool even = ((rc.gid & 1ull) == 0ull);      // uniform: a0 and a_lo are even
         for (uint32_t it = (uint32_t)((a - a_lo) >> 1); a < a_hi; a += 2, ++it) {
-          float oa[CPT], ob[CPT];
+          float oa[4], ob[4];
           const bool has_b = (a + 1 < a_hi);
           if (has_b && !((only >> (it & 31u)) & 1u)) {      // warp-uniform
             cursor_advance(rc, stride);
@@ -696,49 +686,20 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
           if (has_b) P::template rates4<false>(ob, regs, pc, cell0, recp + P::REC, inner_s, dummy);
           if (const unsigned nm = s_slot[s].nanmask; nm != 0u) {        // NaN position -> zero rates (Neurons.py:163-164)
 #pragma unroll
-            for (int i = 0; i < CPT; ++i) {
+            for (int i = 0; i < 4; ++i) {
               if ((nm >> a) & 1u) oa[i] = 0.f;
               if (has_b && ((nm >> (a + 1)) & 1u)) ob[i] = 0.f;
             }
           }
-          if constexpr (CPT == 4) {
-            store4<NOISE>(oa, out, tc, rc, 0);
-            if (has_b) store4<NOISE>(ob, out, tc, rc, out.ld);
-            if (DENSE && (!NOISE || rc.spk != nullptr)) {
-              if (has_b && even) {
-                uint32_t c[4], bl[4];
-                spike_words(c, out, tc, rc.gid);
-                const float nv = spike_neg_dither(c);
-                spike_ballots<true>(bl, c[0], c[1], nv, oa, q16, tc.vmask, true);
-                spike_store(bl, rc.spk);
-                spike_ballots<true>(bl, c[2], c[3], nv, ob, q16, tc.vmask, true);
-                spike_store(bl, rc.spk + out.spike_ld);
-              } else {
-                spikes1(oa, out, tc, rc);
-                if (has_b) {
-                  RowCursor rb = rc;
-                  rb.gid += 1; rb.spk += out.spike_ld;
-                  spikes1(ob, out, tc, rb);
-                }
-              }
-            }
-          } else {
-            // 2 cells per thread (launched only for 8-byte aligned rows and even cell counts, no noise, no dense spikes)
-            if (tc.full4) {
-              st_cs_fv<CPT>(rc.dst, oa);
-              if (has_b) st_cs_fv<CPT>(rc.dst + out.ld, ob);
-            } else {
-#pragma unroll
-              for (int i = 0; i < CPT; ++i)
-                if ((tc.vmask >> i) & 1u) { st_cs_f1(rc.dst + i, oa[i]); if (has_b) st_cs_f1(rc.dst + out.ld + i, ob[i]); }
-            }
-          }
+          store4<NOISE>(oa, out, tc, rc, 0);
+          if (has_b) store4<NOISE>(ob, out, tc, rc, out.ld);
+          if (DENSE && (!NOISE || rc.spk != nullptr)) spikes_pair(oa, ob, has_b, even, out, tc, rc, q16);
           cursor_advance(rc, stride);
           recp += 2 * P::REC;
         }
         if (SPK == 2) {
           __syncwarp();      // orders this warp's rate stores before the read-back
-          if constexpr (CPT == 4) thin_block(&out, tc.cell0, tc.n_cells, tc.c2, tc.c3_spk, out.rates, out.spikes, a0 + a_lo, a_hi - a_lo);
+          thin_block(&out, tc.cell0, tc.n_cells, tc.c2, tc.c3_spk, out.rates, out.spikes, a0 + a_lo, a_hi - a_lo);
         }
       }
     }
@@ -747,67 +708,55 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
   }
 }
 
-// Out-of-line repairs of one ring slot for consumer_fast (rare): pairs whose float32 line-of-sight decision fell inside the
-// band (bit `it` of redo) are re-evaluated with the exact float64 fall-back, and an odd last agent gets its row.  A real
-// call: its register needs must not shape the allocation of the hot loop (the arguments travel through the stack).
+// Repairs of one ring slot for consumer_fast, after its pair loop (rare): pairs whose float32 line-of-sight decision fell
+// inside the band (bit `it` of redo) are re-evaluated with the exact float64 fall-back, and an odd last agent gets its row.
+// Inlined like the pair loop; only the float64 fall-back (place_blocked_exact4) is an out-of-line call.
 template <class P, bool DENSE>
 __device__ __forceinline__ void slot_fixups(const typename P::Regs& regs, const typename P::Const& pc, const OutK& out,
                                             const TailCtx& tc, const float* rec, const uint32_t inner_s, float* d,
                                             uint32_t* spikes, const long long a0, const int n_agents, const uint32_t redo,
                                             const bool act) {
-  constexpr int CPT = P::CPT;
   for (int a = 0; a < n_agents; a += 2, d += 2 * out.ld, rec += 2 * P::REC) {
     const bool has_b = a + 1 < n_agents;
     if (has_b && !((redo >> (a >> 1)) & 1u)) continue;              // warp-uniform
-    float oa[CPT], ob[CPT];
+    float oa[4], ob[4];
     bool dummy = false;
     P::template rates4<false>(oa, regs, pc, tc.cell0, rec, inner_s, dummy);
     if (has_b) P::template rates4<false>(ob, regs, pc, tc.cell0, rec + P::REC, inner_s, dummy);
     if (act) {
-      st_cs_fv<CPT>(d, oa);
-      if (has_b) st_cs_fv<CPT>(d + out.ld, ob);
+      st_cs_f4(d, oa);
+      if (has_b) st_cs_f4(d + out.ld, ob);
     }
-    if constexpr (DENSE && CPT == 4) {                              // whole warp: ballots
+    if constexpr (DENSE) {                                          // whole warp: ballots
       RowCursor rc;
       rc.gid = (unsigned long long)(out.id_offset + a0 + a);
       rc.spk = spikes + (a0 + a) * out.spike_ld + ((tc.cell0 >> 7) << 2);
-      const float q16 = out.dt * 65536.0f;
-      if (has_b) {
-        uint32_t c[4], bl[4];
-        spike_words(c, out, tc, rc.gid);
-        const float nv = spike_neg_dither(c);
-        spike_ballots<true>(bl, c[0], c[1], nv, oa, q16, tc.vmask, true);
-        spike_store(bl, rc.spk);
-        spike_ballots<true>(bl, c[2], c[3], nv, ob, q16, tc.vmask, true);
-        spike_store(bl, rc.spk + out.spike_ld);
-      } else {
-        spikes1(oa, out, tc, rc);
-      }
+      spikes_pair(oa, ob, has_b, true, out, tc, rc, out.dt * 65536.0f);   // even: consumer_fast's tiles start on even ids
     }
   }
 }
 
-// The consumers' slot loop for the common case: no OU noise, no dense spike stream, vector-aligned rows, whole 4-cell
-// groups, all cells resident in one set of registers (n_pad <= 512 * CPT).  Pointers advance incrementally, the rare
-// repairs are a real call (slot_fixups), thinned spikes are a post-pass per slot (thin_block).
+// The consumers' slot loop for the common case: no OU noise, vector-aligned rows, whole 4-cell groups, all cells resident
+// in one set of registers (n_pad <= 2048), an even first global id when there are spikes.  Pointers advance incrementally,
+// the rare repairs run after the pair loop (slot_fixups), thinned spikes are a post-pass per slot (thin_block).
 template <class P, int SPK, class C, int EXP, bool MULTI>
 __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const OutK& out, const RunK& run, StepSlot<P::REC>* s_slot,
                                               uint64_t* s_full, uint64_t* s_empty, const double* s_walls, const long long nq,
                                               const int ctid, const int lane, const long long n_rows) {
-  constexpr int NS = ring_slots<P, C>(), MW = C::MW, NSP = NS / MW, CPT = P::CPT;
-  const int CT = pc.n_pad / CPT;                      // cell-threads needed (multiple of 32, <= RW * 32)
+  constexpr int NS = ring_slots<P, C>(), MW = C::MW, NSP = NS / MW;
+  const int CT = pc.n_pad / 4;                        // cell-threads needed (multiple of 32, <= RW * 32)
   const int G = lean_groups(CT, NS), grp = ctid / CT; // groups of CT threads; group g consumes the tiles q = g, g + G, ...
   if (grp >= G) return;                               // spare warps (the slots' release count is one group's warps)
   constexpr int a_lo = 0;
   typename P::Regs regs;
-  const int cell0 = (ctid % CT) * CPT;
+  const int cell0 = (ctid % CT) * 4;
   TailCtx tc;
   P::load(regs, pc, cell0);
-  tail_init<CPT>(tc, out, cell0, pc.n_cells);
-  const bool act = cell0 < pc.n_cells;                // all CPT cells exist or none (n_cells % 4 == 0)
+  tail_init(tc, out, cell0, pc.n_cells, out.step);
+  const bool act = cell0 < pc.n_cells;                // all 4 cells exist or none (n_cells % 4 == 0)
   const uint32_t inner_s = smem_u32(s_walls) + 32u * (uint32_t)P::wall0(pc);
   const long long ld = out.ld;
-  [[maybe_unused]] const float q16 = out.dt * 65536.0f;
+  const float q16 = out.dt * 65536.0f;
   const long long a_first = ((long long)blockIdx.x + (long long)grp * gridDim.x) * out.tile_agents;   // first row of the group's first tile
   const long long a_step = (long long)G * gridDim.x * out.tile_agents, slot_step = a_step * ld;
   const long long n_steps = MULTI ? run.n_steps : 1;
@@ -819,7 +768,7 @@ __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const
       const long long slot = (run.ring_next + st) % run.ring_rows;
       rates = run.rates_ring + slot * n_rows * ld;
       spikes = run.spikes_ring ? run.spikes_ring + slot * n_rows * out.spike_ld : nullptr;
-      tail_init<CPT>(tc, out, cell0, pc.n_cells, out.step + (unsigned long long)st);
+      tail_init(tc, out, cell0, pc.n_cells, out.step + (unsigned long long)st);
     }
     long long a0 = a_first;
     float* dst0 = rates + a0 * ld + cell0;
@@ -836,51 +785,24 @@ __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const
         float* d = dst0;
         uint32_t redo = 0u;
         const int n2 = (a_hi - a_lo) >> 1;
-        [[maybe_unused]] uint32_t* spk = nullptr;
-        [[maybe_unused]] unsigned long long pair = 0ull;
+        uint32_t* spk = nullptr;
+        unsigned long long pair = 0ull;
         if constexpr (SPK == 1) {
           spk = spikes + a0 * out.spike_ld + ((cell0 >> 7) << 2);
           pair = (unsigned long long)(out.id_offset + a0) >> 1;          // even first global id: rows (2p, 2p+1) are one pair
         }
-        for (int it = 0; it < n2; ++it) {
-          float o[CPT];
-          bool unsure = false;
-          P::template rates4<true, EXP>(o, regs, pc, cell0, recp, inner_s, unsure);
-          if (act) st_cs_fv<CPT>(d, o);
-          [[maybe_unused]] uint32_t c[4], bl[4];
-          [[maybe_unused]] float nv = 0.f;
-          if constexpr (SPK == 1) {
-            // dense spike stream: one Philox4x32-7 call per (agent pair, 4-cell group), a threshold test per rate
-            c[0] = (uint32_t)pair; c[1] = tc.sub ^ ((uint32_t)(pair >> 32) << 24); c[2] = tc.c2; c[3] = tc.c3_spk;
-            philox_keyed<7>(c, out.rk7);
-            nv = spike_neg_dither(c);
-            spike_ballots<false, P::XU_BOUND>(bl, c[0], c[1], nv, o, q16, 0u, act);
-            spike_store(bl, spk);
-          }
-          P::template rates4<true, EXP>(o, regs, pc, cell0, recp + P::REC, inner_s, unsure);
-          if (act) st_cs_fv<CPT>(d + ld, o);
-          if constexpr (SPK == 1) {
-            spike_ballots<false, P::XU_BOUND>(bl, c[2], c[3], nv, o, q16, 0u, act);
-            spike_store(bl, spk + out.spike_ld);
-            spk += 2 * out.spike_ld;
-            pair += 1ull;
-          }
-          redo |= (unsure ? 1u : 0u) << it;
-          d += 2 * ld;
-          recp += 2 * P::REC;
-        }
+        consume_pairs<P, SPK == 1, EXP>(n2, regs, pc, out, tc, cell0, recp, inner_s, ld, d, spk, pair, act, q16, redo);
         redo = __reduce_or_sync(0xffffffffu, redo);
         if (redo != 0u || ((a_hi - a_lo) & 1)) {
-          const typename P::Regs rcopy = regs;            // stack copies, made on this path only
+          // copies: passing regs / pc themselves leaves every kernel's register and stack use as it is, but ptxas then
+          // schedules 65 of the k_step instantiations differently; they stay until a measurement says which is faster
+          const typename P::Regs rcopy = regs;
           const typename P::Const pcopy = pc;
           slot_fixups<P, SPK == 1>(rcopy, pcopy, out, tc, s_slot[s].rec[a_lo], inner_s, dst0, spikes, a0, a_hi - a_lo, redo, act);
         }
         if (const unsigned nm = s_slot[s].nanmask; nm != 0u && act) {     // NaN position -> zero rates (Neurons.py:163-164)
-          float z[CPT];
-#pragma unroll
-          for (int i = 0; i < CPT; ++i) z[i] = 0.f;
           for (int a = a_lo; a < a_hi; ++a)
-            if ((nm >> a) & 1u) st_cs_fv<CPT>(dst0 + (long long)(a - a_lo) * ld, z);
+            if ((nm >> a) & 1u) st_cs_f4(dst0 + (long long)(a - a_lo) * ld, 0.f, 0.f, 0.f, 0.f);
         }
         if constexpr (SPK == 2) {
           __syncwarp();                                  // this warp's rate stores before the read-back
@@ -891,6 +813,23 @@ __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const
       if (lane == 0) mbar_arrive(&s_empty[s]);
     }
   }
+}
+
+// A producer warp publishes the records its lanes < na have written into ring slot `slot`: lane 0 stores the count and the
+// NaN-position mask (Neurons.py:163-164: those agents get zero rates), then the warp arrives on the slot's full barrier.
+template <int REC>
+__device__ __forceinline__ void publish_slot(StepSlot<REC>& slot, uint64_t* full, const int lane, const int na, const bool nanpos) {
+  const unsigned nanmask = __ballot_sync(0xffffffffu, nanpos);
+  if (lane == 0) { slot.na = na; slot.nanmask = nanmask; }
+  __syncwarp();
+  if (lane == 0) mbar_arrive(full);
+}
+
+// Thinned spikes: a producer lane clears its agent's spike row before the tile is published; the consumers OR accepted bits
+// in after that (the mbarrier release / acquire orders these stores before their RED.ORs).
+__device__ __forceinline__ void clear_spike_row(uint32_t* row, const long long words) {
+  for (long long w = 0; w < words; w += 4)
+    asm volatile("st.global.cs.v4.u32 [%0], {%1,%1,%1,%1};" ::"l"(row + w), "r"(0u) : "memory");
 }
 
 // SPK: 0 no spikes, 1 dense spike stream (in the loops), 2 thinned spikes (thin_block per ring slot)
@@ -905,13 +844,13 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
   __shared__ StepSlot<P::REC> s_slot[NS];
   __shared__ uint64_t s_bar, s_full[NS], s_empty[NS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // lean consumers (consumer_fast): every ring slot is consumed by ONE group of warps (n_pad / CPT threads), the general
+  // lean consumers (consumer_fast): every ring slot is consumed by ONE group of warps (n_pad / 4 threads), the general
   // loop (consumer_slots) by all RW consumer warps
   bool lean = false;
-  if constexpr (!NOISE && (SPK != 1 || P::CPT == 4))
-    lean = out.vec_ok && ((pc.n_cells & 3) == 0) && (pc.n_pad <= RW * 32 * P::CPT) && (out.spikes == nullptr || ((out.id_offset & 1ll) == 0));
+  if constexpr (!NOISE)
+    lean = out.vec_ok && ((pc.n_cells & 3) == 0) && (pc.n_pad <= RW * 32 * 4) && (out.spikes == nullptr || ((out.id_offset & 1ll) == 0));
   if (threadIdx.x == 0) {
-    const uint32_t n_release = lean ? (uint32_t)((pc.n_pad / P::CPT) >> 5) : (uint32_t)RW;
+    const uint32_t n_release = lean ? (uint32_t)((pc.n_pad / 4) >> 5) : (uint32_t)RW;
     for (int i = 0; i < NS; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], n_release); }
     mbar_fence_init();
   }
@@ -924,16 +863,10 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
   const long long n_tiles = (n_rows + ta - 1) / ta;
   const long long nq = (n_tiles > (long long)blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
-#ifdef RIAB_PRODUCERS_FIRST
-  const bool producer = warp < MW;
-  const int pw = warp, ctid0 = MW * 32;
-#else
   // producers take the HIGHEST warp ids: the issue arbiter prefers higher warp ids among eligible warps, and
   // the float64 motion chain (one instruction every ~20 cycles) must not wait behind 4 busy consumers
-  const bool producer = warp >= RW;
-  const int pw = warp - RW, ctid0 = 0;
-#endif
-  if (producer) {
+  const int pw = warp - RW;
+  if (warp >= RW) {
     // ------------------------------------------------------------- producers
     reg_set<C::REGS_PRODUCER, C::REGS_LAUNCH>();
     if constexpr (MODE == 3) {
@@ -944,7 +877,6 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
       // its clear of a tile's spike rows for step s+1 may overlap the ORs of up to NSP - 1 earlier steps of that tile, so
       // those steps must have other rows: riab_run launches whole runs with spikes only for ring_rows >= 2 >= NSP
       static_assert(NSP <= 2, "riab_run launches whole runs with spike rings of 2 rows");
-      const long long npw = (nq > pw) ? (nq - pw + MW - 1) / MW : 0;
       long long n = 0;
       for (long long st = 0; st < run.n_steps; ++st) {
         riab_step_io io_st = io;
@@ -956,11 +888,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
           mbar_wait(&s_empty[s], (uint32_t)(((n / NSP) & 1) ^ 1));
           const long long a0 = ((long long)blockIdx.x + q * gridDim.x) * ta;
           const int na = (int)((n_rows - a0) < ta ? (n_rows - a0) : ta);
-          if (SPK == 2 && lane < na && spikes_st != nullptr) {
-            uint32_t* z = spikes_st + (a0 + lane) * out.spike_ld;
-            for (long long w = 0; w < out.spike_ld; w += 4)
-              asm volatile("st.global.cs.v4.u32 [%0], {%1,%1,%1,%1};" ::"l"(z + w), "r"(0u) : "memory");
-          }
+          if (SPK == 2 && lane < na && spikes_st != nullptr) clear_spike_row(spikes_st + (a0 + lane) * out.spike_ld, out.spike_ld);
           bool nanpos = false;
           if (lane < na) {
             AgentState as;
@@ -968,78 +896,63 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             nanpos = (as.px != as.px);
             P::record(s_slot[s].rec[lane], as.px, as.py, as.hdx, as.hdy, s_walls, s_aux, pc, env);
           }
-          const unsigned nanmask = __ballot_sync(0xffffffffu, nanpos);
-          if (lane == 0) { s_slot[s].na = na; s_slot[s].nanmask = nanmask; }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_full[s]);
+          publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
         }
       }
-      return;
-    }
-    for (long long q = pw; q < nq; q += MW) {
-      const int s = (int)(q % NS);
-      const uint32_t k = (uint32_t)(q / NS);
-      mbar_wait(&s_empty[s], (k & 1u) ^ 1u);
-      const long long tile = (long long)blockIdx.x + q * gridDim.x;
-      const long long a0 = tile * ta;
-      const int na = (int)((n_rows - a0) < ta ? (n_rows - a0) : ta);
-      if (SPK == 2 && lane < na) {
-        // thinned spikes: clear the tile's spike rows; the consumers OR accepted bits in after the slot is published
-        // (mbarrier release / acquire orders these stores before their RED.ORs)
-        uint32_t* z = out.spikes + (a0 + lane) * out.spike_ld;
-        for (long long w = 0; w < out.spike_ld; w += 4)
-          asm volatile("st.global.cs.v4.u32 [%0], {%1,%1,%1,%1};" ::"l"(z + w), "r"(0u) : "memory");
-      }
-      if (MODE == 2) {
-        // skewed: publish the records of the CURRENT positions first, then advance the agents
-        // (the next launch's rates) -- consumers never wait for the float64 motion chain.
+    } else {
+      for (long long q = pw; q < nq; q += MW) {
+        const int s = (int)(q % NS);
+        const uint32_t k = (uint32_t)(q / NS);
+        mbar_wait(&s_empty[s], (k & 1u) ^ 1u);
+        const long long tile = (long long)blockIdx.x + q * gridDim.x;
+        const long long a0 = tile * ta;
+        const int na = (int)((n_rows - a0) < ta ? (n_rows - a0) : ta);
+        if (SPK == 2 && lane < na) clear_spike_row(out.spikes + (a0 + lane) * out.spike_ld, out.spike_ld);
+        if (MODE == 2) {
+          // skewed: publish the records of the CURRENT positions first, then advance the agents
+          // (the next launch's rates) -- consumers never wait for the float64 motion chain.
+          bool nanpos = false;
+          if (lane < na) {
+            const long long i = a0 + lane;
+            const double px = ag.pos[2 * i], py = ag.pos[2 * i + 1];
+            nanpos = (px != px);
+            P::record(s_slot[s].rec[lane], px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], s_walls, s_aux, pc, env);
+          }
+          publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
+          if (lane < na) {
+            AgentState st;
+            agent_update_one<false>(ag, mp, md, io, env, s_walls, a0 + lane, st);
+          }
+          continue;
+        }
         bool nanpos = false;
         if (lane < na) {
           const long long i = a0 + lane;
-          const double px = ag.pos[2 * i], py = ag.pos[2 * i + 1];
+          double px, py, hdx = 1.0, hdy = 0.0;
+          if (MODE == 1) {
+            AgentState st;
+            agent_update_one<false>(ag, mp, md, io, env, s_walls, i, st);
+            px = st.px; py = st.py; hdx = st.hdx; hdy = st.hdy;
+          } else {
+            px = pos_in[2 * i]; py = pos_in[2 * i + 1];
+            const double* hd = P::head_dir(pc);                 // egocentric cells evaluated at given positions
+            if (hd != nullptr) { hdx = hd[2 * i]; hdy = hd[2 * i + 1]; }
+          }
           nanpos = (px != px);
-          P::record(s_slot[s].rec[lane], px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], s_walls, s_aux, pc, env);
+          P::record(s_slot[s].rec[lane], px, py, hdx, hdy, s_walls, s_aux, pc, env);
         }
-        const unsigned nanmask = __ballot_sync(0xffffffffu, nanpos);
-        if (lane == 0) { s_slot[s].na = na; s_slot[s].nanmask = nanmask; }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_full[s]);
-        if (lane < na) {
-          AgentState st;
-          agent_update_one<false>(ag, mp, md, io, env, s_walls, a0 + lane, st);
-        }
-        continue;
+        publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
       }
-      bool nanpos = false;
-      if (lane < na) {
-        const long long i = a0 + lane;
-        double px, py, hdx = 1.0, hdy = 0.0;
-        if (MODE == 1) {
-          AgentState st;
-          agent_update_one<false>(ag, mp, md, io, env, s_walls, i, st);
-          px = st.px; py = st.py; hdx = st.hdx; hdy = st.hdy;
-        } else {
-          px = pos_in[2 * i]; py = pos_in[2 * i + 1];
-          const double* hd = P::head_dir(pc);                 // egocentric cells evaluated at given positions
-          if (hd != nullptr) { hdx = hd[2 * i]; hdy = hd[2 * i + 1]; }
-        }
-        nanpos = (px != px);
-        P::record(s_slot[s].rec[lane], px, py, hdx, hdy, s_walls, s_aux, pc, env);
-      }
-      const unsigned nanmask = __ballot_sync(0xffffffffu, nanpos);
-      if (lane == 0) { s_slot[s].na = na; s_slot[s].nanmask = nanmask; }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_full[s]);
     }
   } else {
     // ------------------------------------------------------------- consumers
     reg_set<C::REGS_CONSUMER, C::REGS_LAUNCH>();
-    const int ctid = threadIdx.x - ctid0;
+    const int ctid = threadIdx.x;
     // one copy of the slot loop per exponent form (0: direct, 1: expanded, 2: expanded + folded scale), chosen once:
     // the cell registers then stay in registers across slots (a run-time switch inside the loop made ptxas park them
     // in local memory around every slot)
     const int ex = P::expanded(pc);
-    if constexpr (!NOISE && (SPK != 1 || P::CPT == 4)) {
+    if constexpr (!NOISE) {
       if (lean) {
         if (ex == 2) consumer_fast<P, SPK, C, 2, MODE == 3>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
         else if (ex == 1) consumer_fast<P, SPK, C, 1, MODE == 3>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
@@ -1167,7 +1080,7 @@ __global__ void __launch_bounds__(NT) k_finish_rows(const OutK out, const int n_
 #pragma unroll
   for (int i = 0; i < 4; ++i) o[i] = (cell0 + i < n_cells) ? out.rates[row * out.ld + cell0 + i] : 0.f;
   TailCtx tc;
-  tail_init(tc, out, cell0, n_cells);
+  tail_init(tc, out, cell0, n_cells, out.step);
   tc.full4 = false;
   RowCursor rc;
   cursor_init(rc, out, tc, row);
@@ -1363,10 +1276,9 @@ __global__ void __launch_bounds__(NT) k_bvc_integrate(const BvcConst bc, const f
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const float u = fmaf(dv[i], sc, -mc);                    // (d - mu_d) * s
-          // gaussian * von Mises.  Moving some of the eight exponentials to the 11-instruction FMA-pipe form (ex2_fma,
-          // -DRIAB_BVC_MUFU_TERMS=7) gained in one build and lost in another (register allocation of the unrolled loop
-          // decides): all eight stay on MUFU.
-          const float e = (i < BVC_MUFU_TERMS) ? ex2f(-u * u) : ex2_fma(-u * u);
+          // gaussian * von Mises.  Moving some of the eight exponentials to an 11-instruction FMA-pipe polynomial gained
+          // in one build and lost in another (register allocation of the unrolled loop decides): all eight stay on MUFU.
+          const float e = ex2f(-u * u);
           acc[i] = fmaf(e, vm, acc[i]);
         }
       }
@@ -1707,7 +1619,7 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   // agents per ring slot: 32 for large batches; small ones get equal shares per (CTA, consumer group)
   OutK outk = out_in;
   {
-    const int ct = pc.n_pad / P::CPT;                                 // cell-threads of one consumer group
+    const int ct = pc.n_pad / 4;                                      // cell-threads of one consumer group
     const int ring = (cfg == 4) ? ring_slots<P, StepCfg<4>>() : (cfg == 8) ? ring_slots<P, StepCfg<8>>() : ring_slots<P, StepCfg<12>>();
     const long long groups = (ct > 0 && ct <= RW * 32) ? (long long)g_num_sms * lean_groups(ct, ring) : (long long)g_num_sms;
     int ta = TA;
@@ -2101,7 +2013,7 @@ int riab_grid_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, c
   riab_agents ag; memset(&ag, 0, sizeof(ag));
   riab_motion_params mp; memset(&mp, 0, sizeof(mp));
   riab_step_io io; memset(&io, 0, sizeof(io));
-  return launch_tile<GridPolicy<4>, 0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
+  return launch_tile<GridPolicy, 0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------ BVC
@@ -2294,7 +2206,7 @@ static int neurons_update_impl(const riab_agents* agents, const riab_env* env, c
     GridConst c;
     if ((rc = make_grid(gc, ek, c)) ||
         (rc = make_out(out, noise, gc->n_cells, dt, agents->id_offset, ok, (double)fmaxf(gc->min_fr, gc->max_fr)))) return rc;
-    return launch_tile<GridPolicy<4>, MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
+    return launch_tile<GridPolicy, MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
   }
   if (cells_kind == RIAB_CELLS_BVC) {
     if (MODE == 2) return fail(RIAB_ERR_UNSUPPORTED, "BVC populations are stepped unskewed");
@@ -2406,7 +2318,7 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
         io0.history_row = nullptr;
         cudaStream_t s = (cudaStream_t)stream;
         if (place) return launch_place<3>(ek, *agents, *prm, io0, pcst, ok, nullptr, A, s, &run);
-        return launch_tile<GridPolicy<4>, 3>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
+        return launch_tile<GridPolicy, 3>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
       }
     }
   }

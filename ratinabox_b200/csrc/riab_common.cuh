@@ -137,44 +137,23 @@ RIAB_DEV void tma_bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes,
                : "memory");
 }
 
-// CPT consecutive floats of a packed array (16- / 8-byte vector load)
-template <int CPT>
-RIAB_DEV void ldv(float (&d)[CPT], const float* __restrict__ p) {
-  if constexpr (CPT == 4) { const float4 v = *reinterpret_cast<const float4*>(p); d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w; }
-  else { const float2 v = *reinterpret_cast<const float2*>(p); d[0] = v.x; d[1] = v.y; }
+// 4 consecutive floats of a packed array (16-byte vector load)
+RIAB_DEV void ldv(float (&d)[4], const float* __restrict__ p) {
+  const float4 v = *reinterpret_cast<const float4*>(p);
+  d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
 }
 
 // Streaming (evict-first) vector stores for the write-once rate rows.
 RIAB_DEV void st_cs_f4(float* p, float a, float b, float c, float d) {
   asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
-RIAB_DEV void st_cs_f2(float* p, float a, float b) { asm volatile("st.global.cs.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(a), "f"(b) : "memory"); }
-template <int CPT>
-RIAB_DEV void st_cs_fv(float* p, const float (&o)[CPT]) {
-  if constexpr (CPT == 4) st_cs_f4(p, o[0], o[1], o[2], o[3]);
-  else st_cs_f2(p, o[0], o[1]);
-}
+RIAB_DEV void st_cs_f4(float* p, const float (&o)[4]) { st_cs_f4(p, o[0], o[1], o[2], o[3]); }
 RIAB_DEV void st_cs_f1(float* p, float a) { asm volatile("st.global.cs.f32 [%0], %1;" ::"l"(p), "f"(a) : "memory"); }
 
 RIAB_DEV float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 2^x for x <= 0 on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f through the 1.5*2^23 trick,
-// degree-5 polynomial for 2^f on [-0.5, 0.5] (max relative error 2.5e-7, ex2.approx's own is ~2e-7), exponent
-// added in the integer domain.  11 instructions; used next to MUFU.EX2 where the MUFU pipe is the limit.
-RIAB_DEV float ex2_fma(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(1.3400433e-3f, f, 9.6760374e-3f);
-  p = fmaf(p, f, 5.5503272e-2f);
-  p = fmaf(p, f, 2.4022107e-1f);
-  p = fmaf(p, f, 6.9314718e-1f);
-  p = fmaf(p, f, 1.0000001f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
 
 // NumPy's floating remainder (result takes the sign of the divisor) -- np.mod

@@ -23,28 +23,25 @@ struct GridConst {
   double cxm, cym;
 };
 
-template <int CPT = 4>
 struct GridCellRegs {
-  float kx[3][CPT], ky[3][CPT], ph[3][CPT];
+  float kx[3][4], ky[3][4], ph[3][4];
 };
 
-template <int CPT>
-RIAB_DEV void grid_load_cells(GridCellRegs<CPT>& r, const GridConst& c, int cell0) {
+RIAB_DEV void grid_load_cells(GridCellRegs& r, const GridConst& c, int cell0) {
   const int np = c.n_pad;
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
-    ldv<CPT>(r.kx[k], c.packed + (3 * k + 0) * np + cell0);
-    ldv<CPT>(r.ky[k], c.packed + (3 * k + 1) * np + cell0);
-    ldv<CPT>(r.ph[k], c.packed + (3 * k + 2) * np + cell0);
+    ldv(r.kx[k], c.packed + (3 * k + 0) * np + cell0);
+    ldv(r.ky[k], c.packed + (3 * k + 1) * np + cell0);
+    ldv(r.ph[k], c.packed + (3 * k + 2) * np + cell0);
   }
 }
 
-template <int CPT>
-RIAB_DEV void grid_rates4(float (&out)[CPT], const GridCellRegs<CPT>& r, const GridConst& c, const float* __restrict__ rec) {
+RIAB_DEV void grid_rates4(float (&out)[4], const GridCellRegs& r, const GridConst& c, const float* __restrict__ rec) {
   const float2 p = *reinterpret_cast<const float2*>(rec);
   const float npx = -p.x, npy = -p.y;
 #pragma unroll
-  for (int h = 0; h < CPT / 2; ++h) {                 // cell pairs: the three phases are 2 FFMA each per rate
+  for (int h = 0; h < 2; ++h) {                       // cell pairs: the three phases are 2 FFMA each per rate
     float s0 = 0.f, s1 = 0.f;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {

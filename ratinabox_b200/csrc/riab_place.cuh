@@ -126,42 +126,42 @@ struct PlaceConst {                  // uniform per launch
   double cxm, cym;
 };
 
-// Per-thread cell registers: CPT consecutive cells (4, or 2 for the high-occupancy consumers of StepCfg2).
-template <int WI, int CPT = 4>
+// Per-thread cell registers: 4 consecutive cells.
+template <int WI>
 struct PlaceCellRegs {
-  float cx[CPT], cy[CPT], k[CPT];
-  float fc[WI > 0 ? WI : 1][CPT], tc[WI > 0 ? WI : 1][CPT], tq[WI > 0 ? WI : 1][CPT];   // tq = 1 - tc
-  float ce0[CPT], ce1[CPT];
+  float cx[4], cy[4], k[4];
+  float fc[WI > 0 ? WI : 1][4], tc[WI > 0 ? WI : 1][4], tq[WI > 0 ? WI : 1][4];   // tq = 1 - tc
+  float ce0[4], ce1[4];
 };
 
-template <int WI, int CPT>
-RIAB_DEV void place_load_cells(PlaceCellRegs<WI, CPT>& r, const PlaceConst& c, int cell0) {
+template <int WI>
+RIAB_DEV void place_load_cells(PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0) {
   const float* base = c.packed;
   const int np = c.n_pad;
-  ldv<CPT>(r.cx, base + cell0);
-  ldv<CPT>(r.cy, base + np + cell0);
-  ldv<CPT>(r.k, base + 2 * np + cell0);
+  ldv(r.cx, base + cell0);
+  ldv(r.cy, base + np + cell0);
+  ldv(r.k, base + 2 * np + cell0);
   if (c.expanded) {                                      // registers hold (2k cx, 2k cy, -k|c|^2) instead of (cx, cy, k)
     const float k2 = -2.f * c.kx;
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) { r.cx[i] *= k2; r.cy[i] *= k2; }
-    ldv<CPT>(r.k, base + 3 * np + cell0);
+    for (int i = 0; i < 4; ++i) { r.cx[i] *= k2; r.cy[i] *= k2; }
+    ldv(r.k, base + 3 * np + cell0);
   }
 #pragma unroll
   for (int j = 0; j < WI; ++j) {
     if (j < c.n_inner) {
-      ldv<CPT>(r.fc[j], base + (4 + 2 * j) * np + cell0);
-      ldv<CPT>(r.tc[j], base + (5 + 2 * j) * np + cell0);
+      ldv(r.fc[j], base + (4 + 2 * j) * np + cell0);
+      ldv(r.tc[j], base + (5 + 2 * j) * np + cell0);
     } else {
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) { r.fc[j][i] = 1.f; r.tc[j][i] = -1.f; }   // dummy wall (see place_agent_record)
+      for (int i = 0; i < 4; ++i) { r.fc[j][i] = 1.f; r.tc[j][i] = -1.f; }   // dummy wall (see place_agent_record)
     }
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) r.tq[j][i] = 1.f - r.tc[j][i];
+    for (int i = 0; i < 4; ++i) r.tq[j][i] = 1.f - r.tc[j][i];
   }
   if (WI > 0 && c.geometry == RIAB_GEOM_GEODESIC) {
-    ldv<CPT>(r.ce0, base + (4 + 2 * c.n_inner) * np + cell0);
-    ldv<CPT>(r.ce1, base + (5 + 2 * c.n_inner) * np + cell0);
+    ldv(r.ce0, base + (4 + 2 * c.n_inner) * np + cell0);
+    ldv(r.ce1, base + (5 + 2 * c.n_inner) * np + cell0);
   }
 }
 
@@ -189,10 +189,10 @@ RIAB_DEV double lds_f64(uint32_t saddr) {
 }
 template <int WI>
 __device__ __noinline__ unsigned place_blocked_exact4(const double* __restrict__ centres64, int n_cells, int n_inner,
-                                                      int cell0, uint32_t rec_s, uint32_t inner_s, int cpt = 4) {
+                                                      int cell0, uint32_t rec_s, uint32_t inner_s) {
   const double px = lds_f64(rec_s + 4u * place_pos64(WI)), py = lds_f64(rec_s + 4u * place_pos64(WI) + 8u);
   unsigned m = 0;
-  for (int i = 0; i < cpt; ++i) {
+  for (int i = 0; i < 4; ++i) {
     const int cell = cell0 + i;
     if (cell >= n_cells) continue;
     const double cx = centres64[2 * cell], cy = centres64[2 * cell + 1];
@@ -212,14 +212,14 @@ __device__ __noinline__ unsigned place_blocked_exact4(const double* __restrict__
 //   unsure  : DEFER = true only ORs the band test into it -- the caller redoes the agents it covers
 //             later with DEFER = false, which tests per agent and takes the exact float64 path at once.
 //   EXP     : 1 = the expanded Gaussian form is known to be on (no branch), 0 = known off, -1 = test c.expanded
-template <int WI, int DESC, bool DEFER, int EXP = -1, int CPT = 4>
-RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, const PlaceConst& c, int cell0,
+template <int WI, int DESC, bool DEFER, int EXP = -1>
+RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0,
                            const float* __restrict__ rec, uint32_t inner_s, bool& unsure_io) {
   const float4 r0 = *reinterpret_cast<const float4*>(rec);          // px, py, ep0 | -k|p|^2, ep1
   // ---- line of sight: pen[i] = 1 if the segment centre_i -> agent crosses an inner wall, else 0
-  float pen[CPT];
+  float pen[4];
 #pragma unroll
-  for (int i = 0; i < CPT; ++i) pen[i] = 0.f;
+  for (int i = 0; i < 4; ++i) pen[i] = 0.f;
   if (WI > 0) {
     // With a = |f_c|, b = |f_p| and q' = -f_c f_p 2^20 (> 0 iff the agent is on the other side of the wall's line):
     //   |D| = a + b,  M' = b t_c + a t_p  (a convex combination of t_p, t_c scaled by |D|),
@@ -232,39 +232,38 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
     // |m3| below band/b => the sign of m3 is not certain in float32: re-evaluate in float64.
     // The select is arithmetic: pen = max(0, max_j m3_j) (NaN -> 0) enters the exponent /
     // the squared distance multiplied by 2^100: any pen above the band (>= ~1e-6 / b) makes the rate exactly 0.
-    float worst[CPT], m3_prev[CPT];                       // worst = max(0, max over walls of m3)
+    float worst[4], m3_prev[4];                           // worst = max(0, max over walls of m3)
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) { worst[i] = 0.f; m3_prev[i] = 0.f; }
+    for (int i = 0; i < 4; ++i) { worst[i] = 0.f; m3_prev[i] = 0.f; }
     bool unsure = DEFER ? unsure_io : false;
 #pragma unroll
     for (int j = 0; j < WI; ++j) {
       const float4 pw = *reinterpret_cast<const float4*>(rec + PLACE_WALL0 + 4 * j);
-      float m3[CPT];
+      float m3[4];
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) {
+      for (int i = 0; i < 4; ++i) {
         const float fc = r.fc[j][i];
         const float X = fmaf(fc, pw.x, r.tc[j][i]);
         const float Y = fmaf(fc, pw.y, r.tq[j][i]);
         m3[i] = fminf(fminf(X, Y), fc * pw.z);
       }
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) {
+      for (int i = 0; i < 4; ++i) {
         if ((j & 1) == 1) worst[i] = fmaxf(fmaxf(worst[i], m3[i]), m3_prev[i]);   // pairs of walls
         else if (j == WI - 1) worst[i] = fmaxf(worst[i], m3[i]);                                    // odd wall count: the last one
         m3_prev[i] = m3[i];
       }
-      float am = fminf(fabsf(m3[0]), fabsf(m3[1]));
-      if constexpr (CPT == 4) am = fminf(fminf(am, fabsf(m3[2])), fabsf(m3[3]));
+      const float am = fminf(fminf(fminf(fabsf(m3[0]), fabsf(m3[1])), fabsf(m3[2])), fabsf(m3[3]));
       unsure = unsure || (am < pw.w);
     }
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) pen[i] = worst[i];
+    for (int i = 0; i < 4; ++i) pen[i] = worst[i];
     if (DEFER) unsure_io = unsure;
     else if (unsure) {                                   // rare: redo the group's flags with the reference's float64 test
       const unsigned m = place_blocked_exact4<WI>(c.centres64, c.n_cells, c.n_inner, cell0,
-                                                  (uint32_t)__cvta_generic_to_shared(rec), inner_s, CPT);
+                                                  (uint32_t)__cvta_generic_to_shared(rec), inner_s);
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) pen[i] = ((m >> i) & 1u) ? 1.f : 0.f;
+      for (int i = 0; i < 4; ++i) pen[i] = ((m >> i) & 1u) ? 1.f : 0.f;
     }
   }
   // ---- Gaussian with one common width, expanded:  -k|c-p|^2 = (-k|c|^2 - k|p|^2) + (2k cx) px + (2k cy) py.
@@ -272,7 +271,7 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
   // where the cancellation costs < 4e-6 relative (make_place).  Blocked pairs: exponent - 1e5 -> rate 0 (d = 1000).
   if (DESC == RIAB_PC_GAUSSIAN && (EXP >= 1 || (EXP < 0 && c.expanded))) {
 #pragma unroll
-    for (int h = 0; h < CPT / 2; ++h) {                   // cell pairs: FADD + 2 (3) FFMA per rate
+    for (int h = 0; h < 2; ++h) {                         // cell pairs: FADD + 2 (3) FFMA per rate
       float t0 = fmaf(r.cy[2 * h], r0.y, fmaf(r.cx[2 * h], r0.x, r.k[2 * h] + r0.z));
       float t1 = fmaf(r.cy[2 * h + 1], r0.y, fmaf(r.cx[2 * h + 1], r0.x, r.k[2 * h + 1] + r0.z));
       if (WI > 0) { t0 = fmaf(pen[2 * h], -PLACE_PEN, t0); t1 = fmaf(pen[2 * h + 1], -PLACE_PEN, t1); }
@@ -282,10 +281,10 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
     }
     return;
   }
-  float d2[CPT];
+  float d2[4];
   if (WI == 0 && c.periodic) {                           // warp-uniform
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) {
+    for (int i = 0; i < 4; ++i) {
       float dx = fabsf(r0.x - r.cx[i]), dy = fabsf(r0.y - r.cy[i]);
       dx = (dx > c.half_f) ? c.scale_f - dx : dx;        // the short way round
       dy = (dy > c.half_f) ? c.scale_f - dy : dy;
@@ -293,26 +292,26 @@ RIAB_DEV void place_rates4(float (&out)[CPT], const PlaceCellRegs<WI, CPT>& r, c
     }
   } else {
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) {
+    for (int i = 0; i < 4; ++i) {
       const float dx = r0.x - r.cx[i], dy = r0.y - r.cy[i];
       d2[i] = fmaf(dy, dy, dx * dx);
     }
   }
   // final squared distances (blocked pairs get a distance >= 1000, Environment.py:730)
-  float dd[CPT];
+  float dd[4];
 #pragma unroll
-  for (int i = 0; i < CPT; ++i) dd[i] = (WI > 0) ? fmaf(pen[i], PLACE_PEN, d2[i]) : d2[i];
+  for (int i = 0; i < 4; ++i) dd[i] = (WI > 0) ? fmaf(pen[i], PLACE_PEN, d2[i]) : d2[i];
   const bool geodesic = (DESC < 0) && (WI > 0) && (c.geometry == RIAB_GEOM_GEODESIC);
   const int desc = (DESC >= 0) ? DESC : c.desc;
   if (desc != RIAB_PC_TOP_HAT && !geodesic) {
 #pragma unroll
-    for (int i = 0; i < CPT; ++i)
+    for (int i = 0; i < 4; ++i)
       out[i] = fmaf(place_profile<DESC>(dd[i], r.k[i], c.desc), c.span, c.min_fr);   // Neurons.py:978-980
     return;
   }
   const float2 ep = make_float2(r0.z, r0.w);
 #pragma unroll
-  for (int i = 0; i < CPT; ++i) {
+  for (int i = 0; i < 4; ++i) {
     const bool blocked = (WI > 0) && (dd[i] != d2[i]);
     float dv = dd[i];
     if (geodesic && blocked) {
