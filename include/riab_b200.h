@@ -240,6 +240,42 @@ int riab_ovc_pack(const double* tuning_distances, const double* tuning_angles, c
 int riab_ovc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_ovc_cells* ovc,
                    const double* head_direction_dev, float* out_dev, int64_t ld_out, void* stream);
 
+/* ----------------------------------------------------------- FeedForwardLayer
+ * Neurons.py:2654-2847: firingrate = phi(sum_l W_l . I_l + biases), W_l the (n, n_in) weights of input layer l
+ * (add_input, :2758-2795) and I_l its firing rates, over a batch of rows (agents or positions).  The activations are
+ * the premade set of utils.activate (utils.py:919-1026); bespoke callables stay on the host side and are refused there. */
+#define RIAB_FFL_MAX_INPUTS 4
+typedef enum { RIAB_ACT_LINEAR = 0, RIAB_ACT_SIGMOID = 1, RIAB_ACT_RELU = 2, RIAB_ACT_TANH = 3, RIAB_ACT_RETANH = 4,
+               RIAB_ACT_SOFTPLUS = 5 /* utils.activate's "softmax": gain * log(1 + exp(x - threshold)), utils.py:1017-1026 */
+} riab_activation;
+typedef struct {
+  const float* w_dev;      /* riab_ffl_pack block of inputs[name]["w"] (Neurons.py:2781-2786): W_hi | W_lo */
+  int32_t n_in;            /* input_layer.n (:2779) */
+  int32_t k_pad;           /* filled by riab_ffl_pack: n_in rounded up to 32 */
+  const float* rows_dev;   /* the input's firing rates, (n_rows, ld) f32 (Neurons.py:2819 / :2822); NULL = zeros (the
+                              input has not been updated yet, Neurons.py:120).  riab_run: the row before its first step */
+  int64_t ld;              /* row stride of rows_dev in floats, a multiple of 4 */
+  int32_t population;      /* riab_run: index of the input in `pops` */
+  int32_t lag;             /* riab_run: 0 = this step's row (input registered before the layer), 1 = the previous one
+                              (registered at or after it, recurrence included): the reference's update order */
+} riab_ffl_input;
+typedef struct {
+  int32_t n_cells;                  /* n */
+  int32_t activation;               /* riab_activation */
+  float act[4];                     /* sigmoid: max_fr, min_fr, mid_x, beta = log(19) / (width_x / 2)  (utils.py:961-979);
+                                       relu / tanh / retanh / softplus: gain, threshold (utils.py:981-1026) */
+  const float* bias_dev;            /* (n) f32 biases (Neurons.py:2749-2750, :2829-2832) */
+  float* prime_dev;                 /* (n_rows, ld) f32 firingrate_prime = phi'(V) (Neurons.py:2839-2845) or NULL */
+  int32_t n_inputs;
+  int32_t reserved;
+  riab_ffl_input inputs[RIAB_FFL_MAX_INPUTS];
+} riab_ffl_cells;
+/* Host-side packing of one float64 weight matrix w (n_cells, n_in), row-major, into the error-compensated float32
+ * operand block: W_hi = tf32(w) then W_lo = tf32(float32(w) - W_hi), each (n_pad, k_pad) row-major with n_pad = n
+ * rounded up to 8 and k_pad = n_in rounded up to 32, pads zero.  Fills meta->n_in / k_pad. */
+int64_t riab_ffl_pack_floats(int32_t n_cells, int32_t n_in);
+int riab_ffl_pack(const double* w_host, int32_t n_cells, int32_t n_in, riab_ffl_input* meta_out, float* out_host);
+
 /* ------------------------------------------------------- Neurons.update extras
  * OU noise (Neurons.py:153-160) and spikes (Neurons.py:681-684) for a block of
  * rates already written to rates_dev.  noise_dev (A,N) f32 state (NULL when
@@ -256,7 +292,8 @@ typedef struct {
  * One launch = Agent.update for every agent + Neurons.update of ONE population
  * (motion -> rates [-> noise] [-> spikes] -> history row).  `cells_kind` selects
  * which of pc / gc / bvc / ovc is read. */
-typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3 } riab_cells_kind;
+typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
+               RIAB_CELLS_FFL = 4 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
   int64_t ld;
@@ -276,14 +313,23 @@ int riab_step_fused(const riab_agents* agents, const riab_env* env, const riab_m
 int riab_neurons_update(const riab_agents* agents, const riab_env* env, int32_t cells_kind, const void* cells,
                         const riab_neuron_noise* noise, const riab_rates_out* out, void* stream);
 
+/* FeedForwardLayer.get_state over n_rows input rows (ffl->inputs[i].rows_dev) -> out->rates_row (n_rows, ld) and
+ * ffl->prime_dev, then OU noise and spikes like every population (noise NULL: rates only).  pos_dev (n_rows, 2) f64 or
+ * NULL: rows whose x is NaN get zeros (+ noise) and keep their prime (Neurons.update, Neurons.py:163-164).  With
+ * RIAB_CELLS_FFL, riab_neurons_update / riab_step_fused call this for the agents' rows and positions. */
+int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
+                   const riab_rates_out* out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
- * Population 0 is fused with the motion kernel, the others use riab_neurons_update.
+ * Population 0 is fused with the motion kernel, the others use riab_neurons_update; FeedForwardLayers
+ * (RIAB_CELLS_FFL) run after every other population of the step, in index order, reading ring rows
+ * (next + s - lag) of their inputs, and an Agent with one keeps this unskewed schedule.
  * History rows go to device rings: row (next + s) % rows for step s. */
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
-  const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* */
+  const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

@@ -453,9 +453,10 @@ class Agent:
         else:
             hist = _lib.AgentHistory(None, 0, 0)
         pops = (_lib.Population * max(1, len(self.Neurons)))()
+        for ns in self.Neurons:
+            ns._reserve_history(n_steps)          # first: a FeedForwardLayer binds the other populations' ring rows
         for i, ns in enumerate(self.Neurons):
-            cells = ns._cells()
-            ns._reserve_history(n_steps)
+            cells = ns._cells_for_run()
             out, nz = ns._fill_out_structs(None, None)
             nz.step = ns._upd
             p = pops[i]

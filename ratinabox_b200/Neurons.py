@@ -74,7 +74,8 @@ class Neurons:
         self._noise = None
         self._t_hist = []
         self._last_slot = None
-        self._upd = 0              # updates of THIS population so far: keys its OU-noise / spike Philox streams
+        self._ring_min = 1         # 2 when a FeedForwardLayer reads this population one step late (its previous row)
+        self._upd = 0             # updates of THIS population so far: keys its OU-noise / spike Philox streams
         self._history_view = _HistoryView(self)
         self._last_history_array_cache_time = None
         self._history_arrays = {}
@@ -97,6 +98,10 @@ class Neurons:
             self._sig = sig
         return self._cstruct
 
+    def _cells_for_run(self):
+        """The struct Agent.run hands to riab_run."""
+        return self._cells()
+
     def _rates_from_positions(self, pos_dev, n_pos, out):
         raise NotImplementedError
 
@@ -116,9 +121,12 @@ class Neurons:
         row_bytes = A * ld * 4
         if self._hist is None:
             cap = int(max(1, min(256, self.history_bytes_limit // row_bytes))) if self.save_history else 1
+            cap = max(cap, self._ring_min)
             self._hist = torch.empty((cap, A, ld), dtype=torch.float32, device=self.device)
             self._spk = torch.zeros((cap, A, words), dtype=torch.int32, device=self.device)
             self._hist_cap = cap
+        elif self._hist_cap < self._ring_min:
+            self._grow_ring(self._ring_min)
         elif self.save_history and self._hist_rows == self._hist_cap and 2 * self._hist_cap * row_bytes <= self.history_bytes_limit:
             cap = self._hist_cap
             new = torch.empty((2 * cap, A, ld), dtype=torch.float32, device=self.device)
@@ -142,9 +150,12 @@ class Neurons:
         need = self._hist_rows + n_more if self.save_history else 1
         if self._hist is None:
             cap = int(max(1, min(max(256, need), limit_rows))) if self.save_history else 1
+            cap = max(cap, self._ring_min)
             self._hist = torch.empty((cap, A, ld), dtype=torch.float32, device=self.device)
             self._spk = torch.zeros((cap, A, words), dtype=torch.int32, device=self.device)
             self._hist_cap = cap
+        elif self._hist_cap < self._ring_min:
+            self._grow_ring(self._ring_min)
         elif need > self._hist_cap and self._hist_rows <= self._hist_cap:
             cap = int(min(max(need, 2 * self._hist_cap), limit_rows))
             if cap > self._hist_cap:
@@ -153,6 +164,15 @@ class Neurons:
                 spk = torch.zeros((cap, A, words), dtype=torch.int32, device=self.device)
                 spk[: self._hist_cap].copy_(self._spk)
                 self._hist, self._spk, self._hist_cap = new, spk, cap
+
+    def _grow_ring(self, cap):
+        """Re-allocate the rings with `cap` rows; rows keep their slot index."""
+        torch = self._torch
+        new = torch.empty((cap,) + tuple(self._hist.shape[1:]), dtype=torch.float32, device=self.device)
+        new[: self._hist_cap].copy_(self._hist)
+        spk = torch.zeros((cap,) + tuple(self._spk.shape[1:]), dtype=torch.int32, device=self.device)
+        spk[: self._hist_cap].copy_(self._spk)
+        self._hist, self._spk, self._hist_cap = new, spk, cap
 
     # -------------------------------------------------------------------- update
     def _fill_out_structs(self, row, spk):
@@ -745,3 +765,217 @@ class FieldOfViewOVCs(ObjectVectorCells):
         p["reference_frame"] = "egocentric"
         assert p["cell_arrangement"] is not None, "cell_arrangement must be set for FOV Neurons"
         super().__init__(Agent, p)
+
+
+# =============================================================================
+class _FflInput(dict):
+    """One entry of ``FeedForwardLayer.inputs`` with the reference's keys (Neurons.py:2781-2788).  ``"I"`` is looked up
+    lazily: it is the input layer's ``firingrate`` as it stands when read, so no step pays a device -> host copy."""
+
+    def __getitem__(self, k):
+        if k == "I":
+            return dict.__getitem__(self, "layer").firingrate
+        return dict.__getitem__(self, k)
+
+    def get(self, k, default=None):
+        return self[k] if k in self else default
+
+
+class FeedForwardLayer(Neurons):
+    """ratinabox.FeedForwardLayer (Neurons.py:2654-2847): firingrate = phi(sum over input layers of w . I + biases).
+
+    Inputs are any populations of the same Agent, other FeedForwardLayers and the layer itself included.  Like the
+    reference's update loop (``[Ns.update() for Ns in Ag.Neurons]``) an input registered before the layer gives this
+    step's rates, one registered at or after it the previous step's (zeros before its first update).  ``inputs[name]["w"]``
+    and ``biases`` are float64 NumPy arrays the user may edit between steps; they are re-packed when their bytes change.
+    The activations are the premade ones of utils.activate (utils.py:919-1026); bespoke callables raise.  The contraction
+    runs as an error-compensated TF32 tensor-core GEMM over the whole batch (csrc/riab_ffl.cuh)."""
+    default_params = {                                              # ratinabox/Neurons.py:2699-2705
+        "n": 10,
+        "input_layers": [],
+        "activation_function": {"activation": "linear"},
+        "name": "FeedForwardLayer",
+        "biases": None,
+    }
+    _cells_kind = _lib.CELLS_FFL
+
+    def __init__(self, Agent, params={}):
+        params = dict(params)
+        if "activation_params" in params:                          # Neurons.py:2712-2715
+            warnings.warn("The parameter 'activation_params' is deprecated. Use 'activation_function' instead.")
+            params["activation_function"] = params.pop("activation_params")
+        super().__init__(Agent, params)
+        assert isinstance(self.input_layers, list), "param['input_layers'] must be a list."
+        if len(self.input_layers) == 0:
+            warnings.warn("No input layers have been provided. Either hand them in in the params dictionary "
+                          "params['input_layers']=[list,of,inputs] or use self.add_input_layer() to add them manually.")
+        self._activation()                                           # refuse bespoke activations at construction
+        self.inputs = {}
+        for layer in self.input_layers:
+            self.add_input(layer)
+        if self.biases is None:
+            self.biases = np.zeros(self.n)
+        self._prime = None
+        self._bias_dev = None
+        self._w_dev = []
+
+    def add_input(self, input_layer, w=None, w_init_scale=1, recurrent=False, **kwargs):
+        """FeedForwardLayer.add_input (Neurons.py:2758-2795), with the reference's weight draw."""
+        if input_layer.Agent is not self.Agent:
+            raise ValueError("a FeedForwardLayer's inputs must belong to its own Agent")
+        n, name = input_layer.n, input_layer.name
+        if name not in self.inputs and len(self.inputs) >= _lib.FFL_MAX_INPUTS:
+            raise NotImplementedError(f"at most {_lib.FFL_MAX_INPUTS} input layers per FeedForwardLayer on the CUDA path")
+        if w is None:
+            w = np.random.normal(loc=0, scale=w_init_scale / np.sqrt(n), size=(self.n, n))
+        entry = _FflInput(layer=input_layer, w=w, w_init=w.copy(), I=None, n=input_layer.n, recurrent=recurrent)
+        entry.update(kwargs)
+        self.inputs[name] = entry
+        if input_layer._population_id >= self._population_id:
+            input_layer._ring_min = 2           # read one step late: its previous row must survive its next update
+
+    def _activation(self):
+        """(riab_activation id, 4 float parameters) of the premade activation dict (utils.activate, utils.py:919-1026)."""
+        af = self.activation_function
+        if not isinstance(af, dict) or "function" in af:
+            raise NotImplementedError("bespoke (callable) activation functions are not supported on the CUDA path: use one "
+                                      "of the premade utils.activate dicts, e.g. {'activation': 'relu', 'gain': 1, 'threshold': 0}")
+        name = af["activation"]
+        assert name in _lib.ACTIVATIONS, f"unknown activation {name!r}"
+        if name == "linear":
+            prm = (0.0, 0.0, 0.0, 0.0)
+        elif name == "sigmoid":                                      # utils.py:961-979
+            a = {"max_fr": 1, "min_fr": 0, "mid_x": 1, "width_x": 2}
+            a.update(af)
+            prm = (a["max_fr"], a["min_fr"], a["mid_x"], np.log((1 - 0.05) / 0.05) / (0.5 * a["width_x"]))
+        else:                                                        # utils.py:981-1026
+            a = {"gain": 1, "threshold": 0}
+            a.update(af)
+            prm = (a["gain"], a["threshold"], 0.0, 0.0)
+        return _lib.ACTIVATIONS[name], tuple(float(x) for x in prm)
+
+    def _signature(self):
+        sig = [self.n, repr(self.activation_function), np.ascontiguousarray(self.biases, dtype=np.float64).tobytes()]
+        for name, e in self.inputs.items():
+            sig += [name, id(e["layer"]), e["layer"].n, np.ascontiguousarray(e["w"], dtype=np.float64).tobytes()]
+        return tuple(sig)
+
+    def _pack(self):
+        act, prm = self._activation()
+        c = _lib.FflCells()
+        c.n_cells, c.activation = self.n, act
+        for i in range(4):
+            c.act[i] = prm[i]
+        b = np.ascontiguousarray(self.biases, dtype=np.float64).reshape(-1)
+        assert b.shape[0] == self.n, f"biases must have shape ({self.n},)"
+        self._bias_dev = self._upload(b.astype(np.float32))
+        c.bias_dev = self._bias_dev.data_ptr()
+        self._w_dev = []
+        for i, (name, e) in enumerate(self.inputs.items()):
+            n_in = e["layer"].n
+            w = np.ascontiguousarray(e["w"], dtype=np.float64)
+            assert w.shape == (self.n, n_in), f"inputs[{name!r}]['w'] must have shape ({self.n}, {n_in})"
+            host = np.zeros(self._lib.riab_ffl_pack_floats(self.n, n_in), dtype=np.float32)
+            _lib.check(self._lib.riab_ffl_pack(_f64p(w), self.n, n_in, C.byref(c.inputs[i]), host.ctypes.data_as(_lib.c_float_p)))
+            dev = self._upload(host)
+            self._w_dev.append(dev)
+            c.inputs[i].w_dev = dev.data_ptr()
+        c.n_inputs = len(self.inputs)
+        return c
+
+    def _slot_ptr(self, layer, slot):
+        if slot is None:
+            return None                   # never updated: the reference's initial zeros (Neurons.py:120)
+        return layer._hist.data_ptr() + slot * self.Agent.n_agents * layer._ld() * 4
+
+    def _cells(self):
+        c = super()._cells()
+        if self._prime is None:
+            self._prime = self._torch.zeros((self.Agent.n_agents, self._ld()), dtype=self._torch.float32, device=self.device)
+        c.prime_dev = self._prime.data_ptr()
+        for i, e in enumerate(self.inputs.values()):
+            layer, meta = e["layer"], c.inputs[i]
+            meta.population = layer._population_id
+            meta.lag = 0 if layer._population_id < self._population_id else 1
+            meta.rows_dev, meta.ld = self._slot_ptr(layer, layer._last_slot), layer._ld()
+        return c
+
+    def _row_buffers(self):
+        # update(): the struct was bound before this layer's next row was taken; a self-recurrent input reads the
+        # previous row, located in the ring as it is after any growth
+        prev = self._last_slot
+        out = super()._row_buffers()
+        for i, e in enumerate(self.inputs.values()):
+            if e["layer"] is self:
+                self._cstruct.inputs[i].rows_dev = self._slot_ptr(self, prev)
+        return out
+
+    def _cells_for_run(self):
+        """Agent.run: the rows read one step late before the run's first step are snapshots (the run may overwrite the
+        ring slot they sit in before the layer reads them)."""
+        c = self._cells()
+        self._run_keep = []
+        for i, e in enumerate(self.inputs.values()):
+            layer = e["layer"]
+            if c.inputs[i].lag == 1 and layer._last_slot is not None:
+                snap = layer._hist[layer._last_slot].clone()
+                self._run_keep.append(snap)
+                c.inputs[i].rows_dev = snap.data_ptr()
+        return c
+
+    @property
+    def firingrate_prime(self):
+        """phi'(V) of the last evaluation at "last" (Neurons.py:2839-2845): (n,) for one agent, else (n_agents, n)."""
+        A = self.Agent.n_agents
+        if self._prime is None:
+            return np.zeros(self.n) if A == 1 else np.zeros((A, self.n))
+        r = self._prime[:, : self.n].cpu().numpy().astype(np.float64)
+        return r[0] if A == 1 else r
+
+    def get_state(self, evaluate_at="last", max_recurrence=None, **kwargs):
+        """FeedForwardLayer.get_state (Neurons.py:2797-2847).  "last" reads the inputs' current rows and refreshes
+        firingrate_prime; anything else evaluates the inputs with get_state(evaluate_at, ...) on the device first (recurrent
+        inputs are skipped once max_recurrence runs out).  Returns (n, n_pos) float64, or with ``return_tensor=True`` the
+        (n_pos, n) float32 device tensor."""
+        torch = self._torch
+        return_tensor = kwargs.pop("return_tensor", False)
+        c = self._cells()
+        if evaluate_at == "last":
+            self.Agent._flush_pending()
+            n_pos = self.Agent.n_agents
+            fc = c
+        else:
+            fc = _lib.FflCells.from_buffer_copy(c)
+            fc.prime_dev = None
+            keep = []
+            if evaluate_at == "all":
+                n_pos = self.Agent.Environment.flattened_discrete_coords.shape[0]
+            elif "pos" in kwargs:
+                n_pos = int(np.asarray(kwargs["pos"]).reshape(-1, 2).shape[0]) if not isinstance(kwargs["pos"], torch.Tensor) \
+                    else int(kwargs["pos"].reshape(-1, 2).shape[0])
+            else:
+                n_pos = self.Agent.n_agents
+            for i, e in enumerate(self.inputs.values()):
+                pass_max = max_recurrence
+                if max_recurrence is not None and e["recurrent"]:
+                    if max_recurrence <= 0:
+                        fc.inputs[i].rows_dev = None                  # skipped: contributes nothing (Neurons.py:2812-2815)
+                        continue
+                    pass_max = max_recurrence - 1
+                I = e["layer"].get_state(evaluate_at, max_recurrence=pass_max, return_tensor=True, **kwargs)
+                if I.dtype != torch.float32 or I.stride(1) != 1 or I.stride(0) % 4 or I.data_ptr() % 16:
+                    ld = (I.shape[1] + 3) // 4 * 4
+                    J = torch.zeros((I.shape[0], ld), dtype=torch.float32, device=self.device)
+                    J[:, : I.shape[1]] = I
+                    I = J
+                assert I.shape[0] == n_pos
+                keep.append(I)
+                fc.inputs[i].rows_dev, fc.inputs[i].ld = I.data_ptr(), I.stride(0)
+        out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
+        ro = _lib.RatesOut()
+        ro.rates_row, ro.ld = out.data_ptr(), self._ld()
+        _lib.check(self._lib.riab_ffl_rates(C.byref(fc), n_pos, None, None, C.byref(ro), self.Agent._stream()))
+        if return_tensor:
+            return out[:, : self.n]
+        r = out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
+        return r[:, 0] if (evaluate_at == "last" and n_pos == 1) else r

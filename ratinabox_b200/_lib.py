@@ -72,6 +72,20 @@ class OvcCells(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+FFL_MAX_INPUTS = 4
+
+
+class FflInput(C.Structure):
+    _fields_ = [("w_dev", C.c_void_p), ("n_in", C.c_int32), ("k_pad", C.c_int32), ("rows_dev", C.c_void_p),
+                ("ld", C.c_int64), ("population", C.c_int32), ("lag", C.c_int32)]
+
+
+class FflCells(C.Structure):
+    _fields_ = [("n_cells", C.c_int32), ("activation", C.c_int32), ("act", C.c_float * 4), ("bias_dev", C.c_void_p),
+                ("prime_dev", C.c_void_p), ("n_inputs", C.c_int32), ("reserved", C.c_int32),
+                ("inputs", FflInput * FFL_MAX_INPUTS)]
+
+
 class HistoryView(C.Structure):
     _fields_ = [("agent_ring", C.c_void_p), ("agent_ring_rows", C.c_int32), ("agent_row0", C.c_int32),
                 ("rates_ring", C.c_void_p), ("rates_ring_rows", C.c_int32), ("rates_row0", C.c_int32),
@@ -102,7 +116,8 @@ class AgentHistory(C.Structure):
 PC_DESCRIPTIONS = {"gaussian": 0, "gaussian_threshold": 1, "diff_of_gaussians": 2, "top_hat": 3, "one_hot": 4}
 WALL_GEOMETRIES = {"euclidean": 0, "line_of_sight": 1, "geodesic": 2}
 GC_DESCRIPTIONS = {"rectified_cosines": 0, "shifted_cosines": 1}
-CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC = 0, 1, 2, 3
+CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL = 0, 1, 2, 3, 4
+ACTIVATIONS = {"linear": 0, "sigmoid": 1, "relu": 2, "tanh": 3, "retanh": 4, "softmax": 5}   # riab_activation
 MAX_REC_ITERS = 4
 
 # name -> (restype, argtypes); every symbol include/riab_b200.h declares
@@ -132,6 +147,10 @@ SYMBOLS = {
                                 C.POINTER(OvcCells), c_float_p]),
     "riab_ovc_rates": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(Env), C.POINTER(OvcCells), C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_void_p]),
+    "riab_ffl_pack_floats": (C.c_int64, [C.c_int32, C.c_int32]),
+    "riab_ffl_pack": (C.c_int, [c_double_p, C.c_int32, C.c_int32, C.POINTER(FflInput), c_float_p]),
+    "riab_ffl_rates": (C.c_int, [C.POINTER(FflCells), C.c_int64, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut),
+                                 C.c_void_p]),
     "riab_step_fused": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                   C.c_int32, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut), C.c_void_p]),
     "riab_neurons_update": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.c_int32, C.c_void_p, C.POINTER(NeuronNoise),

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "riab_bvc.cuh"
+#include "riab_ffl.cuh"
 #include "riab_ovc.cuh"
 #include "riab_grid.cuh"
 #include "riab_motion.cuh"
@@ -1802,6 +1803,88 @@ int launch_bvc(const EnvK& env, const riab_agents& ag, const riab_motion_params&
   return 0;
 }
 
+// ---------------------------------------------------------------------------
+// FeedForwardLayer (riab_ffl.cuh).  cuTensorMapEncodeTiled comes from the driver through the runtime's entry-point query,
+// so the library links against the runtime only.
+using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+int ffl_tmap(CUtensorMap* map, const float* base, long long inner, long long outer, long long ld, int box_outer) {
+  static EncodeTiledFn encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    RIAB_CUDA_OK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    if (q != cudaDriverEntryPointSuccess || fn == nullptr) return fail(RIAB_ERR_CUDA, "cuTensorMapEncodeTiled not found");
+    encode = (EncodeTiledFn)fn;
+  }
+  if (((uintptr_t)base) % 16 != 0 || (ld * 4) % 16 != 0) return fail(RIAB_ERR_INVALID, "FFL operands need 16-byte aligned rows");
+  const cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+  const cuuint32_t box[2] = {(cuuint32_t)FFL_BK, (cuuint32_t)box_outer};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(RIAB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
+  return 0;
+}
+
+template <int BN>
+int launch_ffl_bn(FflK& k, cudaStream_t s) {
+  constexpr int smem = ffl_smem_bytes<BN>();
+  RIAB_CUDA_OK(cudaFuncSetAttribute(k_ffl<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k.n_tiles = (k.n_cells + BN - 1) / BN;
+  const long long m_tiles = (k.n_rows + FFL_BM - 1) / FFL_BM;
+  k_ffl<BN><<<(unsigned)(m_tiles * k.n_tiles), FFL_THREADS, smem, s>>>(k);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// One FeedForwardLayer evaluation over n_rows rows (+ noise / spikes through the k_finish_rows post-pass).
+int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, const OutK& out, cudaStream_t s) {
+  if (f == nullptr || f->bias_dev == nullptr) return fail(RIAB_ERR_INVALID, "ffl / bias_dev NULL");
+  if (f->n_cells <= 0) return fail(RIAB_ERR_INVALID, "ffl: n_cells must be > 0");
+  if (f->n_inputs < 0 || f->n_inputs > RIAB_FFL_MAX_INPUTS)
+    return fail(RIAB_ERR_UNSUPPORTED, "ffl: %d inputs (at most %d)", f->n_inputs, RIAB_FFL_MAX_INPUTS);
+  if (f->activation < RIAB_ACT_LINEAR || f->activation > RIAB_ACT_SOFTPLUS) return fail(RIAB_ERR_INVALID, "ffl: bad activation %d", f->activation);
+  if (f->prime_dev != nullptr && out.ld % 4 != 0) return fail(RIAB_ERR_INVALID, "ffl: ld must be a multiple of 4");
+  if (n_rows == 0) return 0;
+  // N tile: the wgmma N of 8, 32 or 64 that wastes least (64: accumulator + per-stage partial = 64 registers)
+  const int bn = f->n_cells <= 8 ? 8 : (f->n_cells <= 32 ? 32 : 64);
+  FflK k;
+  memset(&k, 0, sizeof(k));
+  int rc;
+  const int n_pad = (f->n_cells + 7) / 8 * 8;
+  for (int i = 0; i < f->n_inputs; ++i) {
+    const riab_ffl_input& in = f->inputs[i];
+    if (in.rows_dev == nullptr) continue;                        // an input that was never updated contributes zeros
+    if (in.w_dev == nullptr || in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || in.ld < in.n_in)
+      return fail(RIAB_ERR_INVALID, "ffl input %d: bad weights / sizes (pack with riab_ffl_pack)", i);
+    const int l = k.n_inputs++;
+    if ((rc = ffl_tmap(&k.in[l], in.rows_dev, in.n_in, n_rows, in.ld, FFL_BM)) ||
+        (rc = ffl_tmap(&k.whi[l], in.w_dev, in.k_pad, n_pad, in.k_pad, bn)) ||
+        (rc = ffl_tmap(&k.wlo[l], in.w_dev + (size_t)n_pad * in.k_pad, in.k_pad, n_pad, in.k_pad, bn))) return rc;
+    k.ktiles[l] = in.k_pad / FFL_BK;
+  }
+  k.n_cells = f->n_cells; k.act = f->activation;
+  k.p0 = f->act[0]; k.p1 = f->act[1]; k.p2 = f->act[2]; k.p3 = f->act[3];
+  k.n_rows = n_rows; k.ld = out.ld;
+  k.rates = out.rates; k.prime = f->prime_dev; k.bias = f->bias_dev; k.pos = pos;
+  if (bn == 8) rc = launch_ffl_bn<8>(k, s);
+  else if (bn == 32) rc = launch_ffl_bn<32>(k, s);
+  else rc = launch_ffl_bn<64>(k, s);
+  if (rc) return rc;
+  if (out.noise != nullptr || out.spikes != nullptr) {
+    const int np128 = (f->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
+    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, f->n_cells, np128, n_rows);
+    g_launches++;
+    RIAB_CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
+
 }  // namespace
 
 // ===========================================================================
@@ -2163,6 +2246,50 @@ int riab_ovc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, co
   return launch_tile<OvcPolicy, 0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
 }
 
+// ------------------------------------------------------------ FeedForwardLayer
+static int ffl_n_pad(int n) { return (n + 7) / 8 * 8; }
+static int ffl_k_pad(int n_in) { return (n_in + FFL_BK - 1) / FFL_BK * FFL_BK; }
+// cvt.rna.tf32.f32 on the host: round to nearest (ties away from zero) to 10 mantissa bits, the low 13 bits cleared
+static float tf32_rna(float x) {
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & ~0x1fffu;
+  float r;
+  memcpy(&r, &u, 4);
+  return r;
+}
+
+int64_t riab_ffl_pack_floats(int32_t n_cells, int32_t n_in) {
+  return 2 * (int64_t)ffl_n_pad(n_cells) * ffl_k_pad(n_in);
+}
+
+int riab_ffl_pack(const double* w, int32_t n, int32_t n_in, riab_ffl_input* meta, float* out) {
+  if (w == nullptr || meta == nullptr || out == nullptr || n <= 0 || n_in <= 0) return fail(RIAB_ERR_INVALID, "riab_ffl_pack: bad argument");
+  const int np = ffl_n_pad(n), kp = ffl_k_pad(n_in);
+  float* hi = out;
+  float* lo = out + (size_t)np * kp;
+  for (int i = 0; i < np; ++i)
+    for (int j = 0; j < kp; ++j) {
+      const size_t o = (size_t)i * kp + j;
+      const float x = (i < n && j < n_in) ? (float)w[(size_t)i * n_in + j] : 0.f;
+      hi[o] = tf32_rna(x);
+      lo[o] = tf32_rna(x - hi[o]);
+    }
+  meta->w_dev = nullptr;
+  meta->n_in = n_in;
+  meta->k_pad = kp;
+  return 0;
+}
+
+int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
+                   const riab_rates_out* out, void* stream) {
+  if (ffl == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_ffl_rates: bad argument");
+  OutK ok;
+  int rc;
+  if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok))) return rc;
+  return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
+}
+
 // ----------------------------------------------------------------- fused step
 // MODE 1: motion + rates of one population; 0: rates for agents->pos as it is; 2: skewed (riab_run).
 }  // extern "C"
@@ -2225,6 +2352,14 @@ static int neurons_update_impl(const riab_agents* agents, const riab_env* env, c
     if ((rc = make_ovc(oc, ek, agents->head_direction, c)) || (rc = make_out(out, noise, oc->n_cells, dt, agents->id_offset, ok))) return rc;
     return launch_tile<OvcPolicy, MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
   }
+  if (cells_kind == RIAB_CELLS_FFL) {
+    if (MODE == 2) return fail(RIAB_ERR_UNSUPPORTED, "FeedForwardLayer populations are stepped unskewed");
+    const riab_ffl_cells* fc = (const riab_ffl_cells*)cells;
+    if ((rc = make_out(out, noise, fc->n_cells, dt, agents->id_offset, ok))) return rc;
+    // the layer reads other populations' rows, not the positions (except for its NaN mask): the motion runs first
+    if (MODE == 1 && (rc = riab_agent_update(agents, env, prm, io, stream))) return rc;
+    return launch_ffl(fc, agents->n_agents, agents->pos, ok, s);
+  }
   return fail(RIAB_ERR_INVALID, "bad cells_kind %d", cells_kind);
 }
 extern "C" {
@@ -2252,8 +2387,12 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
   // float64 motion chain never gates the rate warps.
   const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
                        ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
-  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && n_steps >= 1 && io->xi == nullptr &&
-                    !io->collision_mask && !io->first_hit && !io->n_iters;
+  // A FeedForwardLayer reads other populations' rows of the same step and masks the agents whose position of that step is
+  // NaN, so an Agent with one keeps the plain schedule: the positions advance before any population of the step.
+  bool any_ffl = false;
+  for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
+  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && !any_ffl && n_steps >= 1 &&
+                    io->xi == nullptr && !io->collision_mask && !io->first_hit && !io->n_iters;
   auto step_io = [&](int64_t st) {
     riab_step_io sio = *io;
     sio.step = io->step + (uint64_t)st;
@@ -2386,10 +2525,13 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
       if ((rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
       continue;
     }
-    // populations 1.. first (they read the positions of step st), population 0 last (it may advance them)
-    for (int pi = 0; pi < n_pops; ++pi) {
-      const int p = skew ? ((pi + 1) % n_pops) : pi;
+    // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
+    // FeedForwardLayers in registration order, after every row they read of this step exists
+    if (!skew && pops[0].kind == RIAB_CELLS_FFL && (rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
+    for (int pi = 0; pi < 2 * n_pops; ++pi) {
+      const int p = pi >= n_pops ? pi - n_pops : (skew ? ((pi + 1) % n_pops) : pi);
       const riab_population& pp = pops[p];
+      if ((pp.kind == RIAB_CELLS_FFL) != (pi >= n_pops)) continue;
       if (pp.rates_ring == nullptr || pp.ring_rows <= 0) return fail(RIAB_ERR_INVALID, "population %d: no rates ring", p);
       const size_t slot = (size_t)((pp.ring_next + st) % pp.ring_rows);
       riab_rates_out ro = pp.out;
@@ -2399,11 +2541,29 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
       else if (pp.kind == RIAB_CELLS_GRID) n_cells = ((const riab_grid_cells*)pp.cells)->n_cells;
       else if (pp.kind == RIAB_CELLS_BVC) n_cells = ((const riab_bvc_cells*)pp.cells)->n_cells;
       else if (pp.kind == RIAB_CELLS_OVC) n_cells = ((const riab_ovc_cells*)pp.cells)->n_cells;
+      else if (pp.kind == RIAB_CELLS_FFL) n_cells = ((const riab_ffl_cells*)pp.cells)->n_cells;
       ro.spikes_row = pp.spikes_ring ? pp.spikes_ring + slot * A * (size_t)(4 * ((n_cells + 127) / 128)) : nullptr;
       riab_neuron_noise nz = pp.noise;
       nz.step = pp.noise.step + (uint64_t)st;
       nz.dt = prm->dt;
-      if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
+      if (pp.kind == RIAB_CELLS_FFL) {
+        // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
+        // previous step's: before the first step, the row the caller passed
+        riab_ffl_cells fc = *(const riab_ffl_cells*)pp.cells;
+        for (int i = 0; i < fc.n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
+          riab_ffl_input& in = fc.inputs[i];
+          if (in.population < 0 || in.population >= n_pops || (in.lag == 0) != (in.population < p) || in.lag < 0 || in.lag > 1)
+            return fail(RIAB_ERR_INVALID, "population %d: FeedForwardLayer input %d (population %d, lag %d) out of order", p, i,
+                        in.population, in.lag);
+          const riab_population& ip = pops[in.population];
+          if (in.lag == 1 && st == 0) continue;
+          if (in.lag == 1 && ip.ring_rows < 2)
+            return fail(RIAB_ERR_INVALID, "population %d feeds a FeedForwardLayer with one step of lag: it needs 2 ring rows", in.population);
+          in.rows_dev = ip.rates_ring + (size_t)((ip.ring_next + st - in.lag) % ip.ring_rows) * A * ip.out.ld;
+          in.ld = ip.out.ld;
+        }
+        rc = riab_neurons_update(agents, env, pp.kind, &fc, &nz, &ro, stream);
+      } else if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
       else if (p == 0 && st + 1 < n_steps) {
         const riab_step_io nxt = step_io(st + 1);          // the motion it runs belongs to step st+1
         rc = neurons_update_impl<2>(agents, env, prm, &nxt, pp.kind, pp.cells, &nz, &ro, stream);
