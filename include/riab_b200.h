@@ -130,6 +130,44 @@ typedef struct {
 int riab_agent_update(const riab_agents* agents, const riab_env* env,
                       const riab_motion_params* prm, const riab_step_io* io, void* stream);
 
+/* ---------------------------------------------------- imported / forced motion
+ * Agent.update's other two branches (Agent.py:202-242): the position of a step comes from an imported trajectory
+ * (Agent.import_trajectory, :543-659: `pos = pos_interp(t % max(t_interp))`, pos_interp the not-a-knot cubic spline of
+ * scipy's interp1d(kind="cubic")) or from a forced_next_position; then measured velocity / rotational velocity with
+ * overwrite_velocity=True (:444-472), head direction, distance travelled (+0 when pos or prev_pos holds a NaN) and the
+ * history row.  The random-motion parameters and drift_velocity are ignored, distance_to_closest_wall is not updated.
+ *
+ * A trajectory: times shared by every agent, positions either shared (n_traj = 1) or one per agent (n_traj = n_agents),
+ * stored sample-major so that the agents' samples of one time are contiguous.  M holds the spline's second
+ * derivatives, written by riab_trajectory_build. */
+typedef struct {
+  const double* times_dev;  /* (T) f64, times[0] == 0, strictly increasing (import_trajectory shifts and sorts) */
+  const double* y_dev;      /* (T, n_traj, 2) f64 positions */
+  double* M_dev;            /* (T, n_traj, 2) f64 second derivatives of the spline */
+  int64_t T;                /* >= 4 (interp1d's minimum for kind="cubic") */
+  int64_t n_traj;           /* 1 (shared) or n_agents */
+  double t_max;             /* times[T-1] = max(t_interp) */
+} riab_trajectory;
+
+/* Solve the not-a-knot spline system of every (trajectory, axis) column (one thread per column) into tr->M_dev.
+ * times_host: the same T times as tr->times_dev; the elimination factors, which depend on the times only, are
+ * computed on the host in float64. */
+int riab_trajectory_build(const riab_trajectory* tr, const double* times_host, void* stream);
+
+typedef enum { RIAB_MOTION_RANDOM = 0, RIAB_MOTION_IMPORTED = 1, RIAB_MOTION_FORCED = 2 } riab_motion_kind;
+typedef struct {
+  int32_t kind;                 /* riab_motion_kind */
+  int32_t forced_broadcast;     /* RIAB_MOTION_FORCED: 1 = forced_dev is one (2) position for every agent */
+  double t;                     /* Agent.t of the (first) step, after its `t += dt`; later steps of a run add dt */
+  riab_trajectory traj;         /* RIAB_MOTION_IMPORTED */
+  const double* forced_dev;     /* RIAB_MOTION_FORCED: (A,2) or (2) f64, device or page-locked host memory */
+} riab_motion_source;
+
+/* Agent.update with a motion source; src == NULL or RIAB_MOTION_RANDOM is riab_agent_update.  io: seed / step (the
+ * zero-displacement draw), history_row, pos_mirror; drift_velocity, xi and the collision taps are ignored. */
+int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
+                          const riab_step_io* io, const riab_motion_source* src, void* stream);
+
 /* ----------------------------------------------------------------- PlaceCells */
 typedef enum { RIAB_PC_GAUSSIAN = 0, RIAB_PC_GAUSSIAN_THRESHOLD = 1, RIAB_PC_DIFF_OF_GAUSSIANS = 2,
                RIAB_PC_TOP_HAT = 3, RIAB_PC_ONE_HOT = 4 } riab_pc_description;   /* Neurons.py:959-976 */
@@ -347,6 +385,14 @@ typedef struct {
 int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
              const riab_population* pops, int32_t n_pops, const riab_agent_history* hist, int64_t n_steps,
              void* stream);
+
+/* riab_run following a motion source (src == NULL or RIAB_MOTION_RANDOM: riab_run).  RIAB_MOTION_IMPORTED: step s
+ * reads the trajectory at (t + dt + ... + dt) % t_max, the clock advanced by `t += dt` like Agent.update.  A single
+ * Place / Grid population runs as one launch where riab_run's would; otherwise every step is the motion kernel followed
+ * by the populations' rates.  RIAB_MOTION_FORCED is refused: a forced position belongs to one step. */
+int riab_run_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
+                 const riab_motion_source* src, const riab_population* pops, int32_t n_pops,
+                 const riab_agent_history* hist, int64_t n_steps, void* stream);
 
 /* ------------------------------------------------------------ history analytics
  * utils.bin_data_for_histogramming (utils.py:544-589) over the device history rings, pooled over agents and steps:

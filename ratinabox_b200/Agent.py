@@ -14,6 +14,10 @@ API parity with the reference (ratinabox/Agent.py):
     they have the reference's shapes ((2,) / scalar); otherwise a leading agent axis.
   * ``history`` / ``get_history_arrays()`` (Agent.py:111-120, :1093-1102), backed by a
     device ring buffer that is only materialised on access.
+  * ``import_trajectory(times, positions, dataset)`` (Agent.py:543-659) and
+    ``update(forced_next_position=...)`` (Agent.py:202-253): the imported / forced branches of
+    Agent.update.  One trajectory for every agent, or one per agent over shared times; its
+    not-a-knot spline is solved on the device (riab_trajectory_build) and ``run()`` follows it.
 
 The launch is lazy: ``update()`` queues the motion step, and the first
 ``Neurons.update()`` that follows runs it fused with its firing rates in one
@@ -132,6 +136,10 @@ class Agent:
         self._drift_host_ptr = None         # pinned drift commands of the queued step (eager stepped API)
         self._pos_copy_inflight = False
         self._motion_event_valid = False
+        self._traj = None                   # imported trajectory: device arrays + riab_trajectory
+        self._src = _lib.MotionSource()     # motion source of the current step
+        self._forced_dev = None
+        self._forced_keep = None
 
         # ---- initial state (Agent.py:523-535, :136-141), sampled on the host like the reference
         pos = Environment.sample_positions(n=A, method="random")
@@ -278,12 +286,137 @@ class Agent:
     # state attributes (properties are generated below the class body)
 
     # -------------------------------------------------------------------- update
+    def import_trajectory(self, times=None, positions=None, dataset=None, interpolate=True):
+        """Agent.import_trajectory (ratinabox/Agent.py:543-659) for every agent.  ``times`` (T,) are shared by all
+        agents; ``positions`` is (T, 2), one trajectory for every agent, or (n_agents, T, 2), one per agent.  update()
+        and run() then move the agents to ``pos_interp(t % max(t_interp))``, pos_interp the not-a-knot cubic spline of
+        scipy's interp1d(kind="cubic"), solved on the device.  ``dataset`` names ``<ratinabox>/data/<dataset>.npz`` of
+        an installed ratinabox package (or is a path to such a file)."""
+        import os
+        import torch
+        if interpolate is not True:
+            raise NotImplementedError("import_trajectory(interpolate=False) is not supported: the reference itself fails "
+                                      "there (Agent.py:657 reads self.pos_interp, which only interpolate=True creates)")
+        self._flush_pending()
+        assert self.Environment.boundary_conditions == "solid", "Only solid boundary conditions are supported"
+        if dataset is not None:
+            if dataset == "sargolini":
+                print(
+                    """Attempting to import Sargolini locomotion dataset.
+                    Please cite Sargolini et al. (2006) DOI:10.1126/science.1125572 if you use this in your work.
+                    The full dataset (along with many more) can be found here https://www.ntnu.edu/kavli/research/grid-cell-data
+                    The exact datafile being used is 8F6BE356-3277-475C-87B1-C7A977632DA7_1/11084-03020501_t2c1.mat"""
+                )
+            try:
+                import ratinabox
+                base = os.path.abspath(os.path.join(ratinabox.__file__, os.pardir))
+            except ImportError:
+                base = os.path.abspath(os.path.join(__file__, os.pardir))
+            dataset = os.path.join(os.path.join(base, "data"), dataset + ".npz")
+            try:
+                data = np.load(dataset)
+            except FileNotFoundError:
+                print(f"IMPORT FAILED. No datafile found at {dataset}. Please try a different one. For now the default "
+                      f"inbuilt random policy will be used.")
+                return
+            times = data["t"]
+            positions = data["pos"]
+            print(f"Successfully imported dataset from {dataset}")
+        else:
+            if (times is not None) and (positions is not None):
+                times, positions = np.array(times), np.array(positions)
+                print("Successfully imported dataset from arrays passed")
+            else:
+                print("No data passed, provided arguments 'times' and 'positions'")
+        times = np.asarray(times, dtype=np.float64)
+        positions = np.asarray(positions, dtype=np.float64)
+        if times.ndim != 1:
+            raise NotImplementedError("per-agent time bases are not supported: pass one (T,) array of times shared by "
+                                      "every agent, with positions (T, 2) or (n_agents, T, 2)")
+        per_agent = positions.ndim == 3
+        if per_agent and positions.shape[0] != self.n_agents:
+            raise ValueError(f"positions of shape {positions.shape}: expected (T, 2) or (n_agents={self.n_agents}, T, 2)")
+        assert (positions.shape[1] if per_agent else len(positions)) == len(times), \
+            "time and position arrays must have same length"
+        times = times - min(times)
+        print(f"Total of {times[-1]:.1f} s of data available")
+        ex = self.Environment.extent
+        positions = positions.reshape(self.n_agents, -1, 2) if per_agent else positions.reshape(-1, 2)
+        px, py = positions[..., 0], positions[..., 1]
+        if (px.max() > ex[1]) or (px.min() < ex[0]) or (py.max() > ex[3]) or (py.min() < ex[2]):
+            print(
+                f"""WARNING: the size of the trajectory is significantly larger than the environment you are using.
+                    The Environment extent is [minx,maxx,miny,maxy]=[{ex[0]:.1f},{ex[1]:.1f},{ex[2]:.1f},{ex[3]:.1f}], whereas extreme coords are [{px.min():.1f},{px.max():.1f},{py.min():.1f},{py.max():.1f}].
+                    Recommended to use larger environment."""
+            )
+        # interp1d's own checks of the sample times (at least 4 for kind="cubic", no duplicates) and its sort
+        from scipy.interpolate import interp1d
+        interp1d(times, np.zeros(len(times)), kind="cubic", fill_value="extrapolate")
+        order = np.argsort(times, kind="mergesort")
+        xs = np.ascontiguousarray(times[order])
+        ys = positions[:, order, :].transpose(1, 0, 2) if per_agent else positions[order][:, None, :]
+        T, n_traj = len(xs), ys.shape[1]
+        need = 32 * T * n_traj + 8 * T
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need > free:
+            raise MemoryError(f"import_trajectory: {n_traj} trajectories of {T} samples need {need / 2**30:.2f} GiB of "
+                              f"device memory (positions and spline coefficients), {free / 2**30:.2f} GiB are free")
+        f64 = dict(dtype=torch.float64, device=self.device)
+        tr = {"times": torch.as_tensor(xs, **f64), "y": torch.as_tensor(np.ascontiguousarray(ys), **f64)}
+        tr["M"] = torch.empty_like(tr["y"])
+        c = _lib.Trajectory()
+        c.times_dev, c.y_dev, c.M_dev = tr["times"].data_ptr(), tr["y"].data_ptr(), tr["M"].data_ptr()
+        c.T, c.n_traj, c.t_max = T, n_traj, float(xs[-1])
+        _lib.check(self._lib.riab_trajectory_build(C.byref(c), xs.ctypes.data_as(_lib.c_double_p), self._stream()))
+        tr["c"] = c
+        self._traj = tr
+        self.interpolate = interpolate
+        self.t_interp = times
+        self.use_imported_trajectory = True
+        # pos = prev_pos = pos_interp(0) (Agent.py:658-659): the first sample
+        self.pos = np.ascontiguousarray(ys[0])
+
+    def _stage_source(self, forced):
+        """Fill self._src for this step: the imported trajectory (which wins over forced_next_position, Agent.py:220-
+        229) or the forced positions.  Returns the motion kind."""
+        import torch
+        src = self._src
+        if self.use_imported_trajectory:
+            src.kind = _lib.MOTION_IMPORTED
+            src.traj = self._traj["c"]
+            src.t = float(self.t)
+            return src.kind
+        src.kind = _lib.MOTION_FORCED
+        if isinstance(forced, torch.Tensor):
+            f = forced
+        else:
+            assert isinstance(forced, np.ndarray), "forced_next_position must be an np.array"       # Agent.py:250
+            f = torch.as_tensor(forced)
+        assert tuple(f.shape) in ((2,), (self.n_agents, 2)), \
+            "forced_next_position must be an np.array of shape Env.D"                                 # Agent.py:251
+        if f.dtype != torch.float64:
+            f = f.to(torch.float64)
+        src.forced_broadcast = 1 if tuple(f.shape) == (2,) else 0
+        if (f.is_cuda or f.is_pinned()) and f.is_contiguous():
+            # device or page-locked host positions are read by the motion kernel itself; like a non_blocking copy, the
+            # buffer must not change before the step has run
+            self._forced_keep = f
+            src.forced_dev = f.data_ptr()
+        else:
+            if self._forced_dev is None or tuple(self._forced_dev.shape) != tuple(f.shape):
+                self._forced_dev = torch.empty(tuple(f.shape), dtype=torch.float64, device=self.device)
+            self._forced_dev.copy_(f, non_blocking=True)
+            src.forced_dev = self._forced_dev.data_ptr()
+        return src.kind
+
     def update(self, dt=None, drift_velocity=None, drift_to_random_strength_ratio=1, **kwargs):
-        """Agent.update (ratinabox/Agent.py:160-242), random-motion branch, for every agent."""
+        """Agent.update (ratinabox/Agent.py:160-242) for every agent: the random-motion branch, or the imported /
+        forced one (import_trajectory, forced_next_position), which ignore drift_velocity and the motion kwargs."""
         import torch
         self._flush_pending()
-        if kwargs.get("forced_next_position", None) is not None or self.use_imported_trajectory:
-            raise NotImplementedError("imported / forced trajectories are outside the CUDA hot path (SURVEY.md section 2 row 8)")
+        forced = kwargs.get("forced_next_position", None)
+        if self.use_imported_trajectory or forced is not None:
+            return self._update_source(dt, forced, kwargs)
         dt = (dt or self.dt)
         self.dt = dt
         self.prev_t = self.t
@@ -375,6 +508,58 @@ class Agent:
         if not self.fused_step and not self._staging_only:
             self._flush_pending()                      # launch the motion kernel now (asynchronous)
 
+    def _fill_motion_params(self, dt, kwargs, drift_to_random_strength_ratio=1):
+        mp = self._mp
+        mp.dt = float(dt)
+        mp.speed_coherence_time_kw = float(kwargs.get("speed_coherence_time", self.speed_coherence_time))
+        mp.speed_mean_kw = float(kwargs.get("speed_mean", self.speed_mean))
+        mp.speed_mean = float(self.speed_mean)
+        mp.speed_std = float(self.speed_std)
+        mp.speed_coherence_time = float(self.speed_coherence_time)
+        mp.rotational_velocity_coherence_time_kw = float(
+            kwargs.get("rotational_velocity_coherence_time", self.rotational_velocity_coherence_time))
+        mp.rotational_velocity_std_kw = float(kwargs.get("rotational_velocity_std", self.rotational_velocity_std))
+        mp.rotational_velocity_drift_kw = float(kwargs.get("rotational_velocity_drift", 0))
+        mp.head_direction_smoothing_timescale = float(self.head_direction_smoothing_timescale)
+        mp.thigmotaxis_kw = float(kwargs.get("thigmotaxis", self.thigmotaxis))
+        mp.wall_repel_distance_kw = float(kwargs.get("wall_repel_distance", self.wall_repel_distance))
+        mp.wall_repel_strength_kw = float(kwargs.get("wall_repel_strength", self.wall_repel_strength))
+        mp.drift_to_random_strength_ratio = float(drift_to_random_strength_ratio)
+
+    def _update_source(self, dt, forced, kwargs):
+        """The imported / forced branches of Agent.update (Agent.py:219-242).  The motion kernel is launched at once
+        (with fused_step too: the rates then take the unfused path), except while run() stages its first step."""
+        if not self.use_imported_trajectory:
+            self._stage_source(forced)          # validates before the clock moves
+        dt = (dt or self.dt)
+        self.dt = dt
+        self.prev_t = self.t
+        self.t += dt
+        self._sync_user_writes()
+        if self.use_imported_trajectory:
+            self._stage_source(None)
+        self._fill_motion_params(dt, kwargs)
+        io = self._io
+        io.drift_velocity = io.xi = None
+        io.collision_mask = io.first_hit = io.n_iters = None
+        io.pos_mirror = None
+        self._tape = self._rec = None
+        self._drift_host_ptr = None
+        io.seed = int(self.seed) & 0xFFFFFFFFFFFFFFFF
+        io.step = self._step
+        io.history_row = None
+        if self.save_history:
+            io.history_row = self._history_row_ptr()
+            self._t_hist.append(self.t)
+        self._pos_mirror_current = False
+        self._motion_event_valid = False
+        self._step += 1
+        if self._staging_only:
+            return
+        self._wait_pos_copy()
+        _lib.check(self._lib.riab_agent_update_src(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
+                                                   C.byref(io), C.byref(self._src), self._stream()))
+
     def _wait_pos_copy(self):
         """Order the compute stream behind an in-flight D2H copy of the positions (it reads what comes next overwrites)."""
         if self._pos_copy_inflight:
@@ -428,6 +613,9 @@ class Agent:
             return
         if "drift_velocity" in kwargs and kwargs["drift_velocity"] is not None:
             raise NotImplementedError("run() is the free-exploration loop; step with update(drift_velocity=...) for control")
+        if kwargs.get("forced_next_position", None) is not None:
+            raise NotImplementedError("run() cannot take forced_next_position: a forced position belongs to one step; "
+                                      "step with update(forced_next_position=...)")
         # stage everything exactly like one update() would, then hand the loop to C
         self._staging_only = True
         try:
@@ -466,9 +654,15 @@ class Agent:
             p.spikes_ring = ns._spk.data_ptr() if (ns.save_history and ns.save_spikes) else None
             p.ring_rows, p.ring_next = ns._hist_cap, ns._hist_rows % ns._hist_cap
         self._io.step = first_step
-        _lib.check(self._lib.riab_run(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
-                                      C.byref(self._io), pops, len(self.Neurons), C.byref(hist), n_steps,
-                                      self._stream()))
+        if self.use_imported_trajectory:
+            # the first step's clock (the staging update() made its `t += dt`); the library advances it per step
+            _lib.check(self._lib.riab_run_src(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
+                                              C.byref(self._io), C.byref(self._src), pops, len(self.Neurons), C.byref(hist),
+                                              n_steps, self._stream()))
+        else:
+            _lib.check(self._lib.riab_run(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
+                                          C.byref(self._io), pops, len(self.Neurons), C.byref(hist), n_steps,
+                                          self._stream()))
         # host-side bookkeeping of the n_steps that just ran: the clock advances by `t += dt` per step like update()
         # (the staging update() above already made the first), so the times equal the stepped loop's bit for bit
         ts = [self.t]

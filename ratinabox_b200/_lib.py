@@ -43,6 +43,19 @@ class StepIO(C.Structure):
                 ("history_row", C.c_void_p), ("pos_mirror", C.c_void_p)]
 
 
+class Trajectory(C.Structure):
+    _fields_ = [("times_dev", C.c_void_p), ("y_dev", C.c_void_p), ("M_dev", C.c_void_p), ("T", C.c_int64),
+                ("n_traj", C.c_int64), ("t_max", C.c_double)]
+
+
+class MotionSource(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("forced_broadcast", C.c_int32), ("t", C.c_double), ("traj", Trajectory),
+                ("forced_dev", C.c_void_p)]
+
+
+MOTION_RANDOM, MOTION_IMPORTED, MOTION_FORCED = 0, 1, 2      # riab_motion_kind
+
+
 class PlaceCells(C.Structure):
     _fields_ = [("n_cells", C.c_int32), ("description", C.c_int32), ("wall_geometry", C.c_int32),
                 ("n_inner_walls", C.c_int32), ("min_fr", C.c_float), ("max_fr", C.c_float),
@@ -129,6 +142,9 @@ SYMBOLS = {
     "riab_history_rate_maps": (C.c_int, [C.POINTER(HistoryView), C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "riab_agent_update": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO), C.c_void_p]),
+    "riab_trajectory_build": (C.c_int, [C.POINTER(Trajectory), c_double_p, C.c_void_p]),
+    "riab_agent_update_src": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
+                                        C.POINTER(MotionSource), C.c_void_p]),
     "riab_place_pack_floats": (C.c_int64, [C.c_int32, C.c_int32]),
     "riab_place_pack": (C.c_int, [c_double_p, c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_int32, c_double_p,
                                   C.c_int32, C.POINTER(PlaceCells), c_float_p]),
@@ -157,6 +173,9 @@ SYMBOLS = {
                                       C.POINTER(RatesOut), C.c_void_p]),
     "riab_run": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                            C.POINTER(Population), C.c_int32, C.POINTER(AgentHistory), C.c_int64, C.c_void_p]),
+    "riab_run_src": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
+                               C.POINTER(MotionSource), C.POINTER(Population), C.c_int32, C.POINTER(AgentHistory), C.c_int64,
+                               C.c_void_p]),
     "riab_agent_update_host": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "riab_positions_wait": (C.c_int, []),

@@ -2,6 +2,8 @@
 //
 // Kernel inventory
 //   k_agent_update      Agent.update, one agent per thread (float64)
+//   k_agent_update_src  Agent.update from an imported trajectory / forced positions, one agent per thread (float64)
+//   k_traj_build        not-a-knot spline of imported trajectories, one thread per (trajectory, axis) column
 //   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells:
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
@@ -24,6 +26,7 @@
 #include "riab_grid.cuh"
 #include "riab_motion.cuh"
 #include "riab_place.cuh"
+#include "riab_traj.cuh"
 
 using namespace riab;
 
@@ -89,6 +92,7 @@ struct RunK {
   long long ring_rows, ring_next;
   float* hist_ring;             // (hist_rows, A, 8) agent history rows or NULL
   long long hist_rows, hist_next;
+  SrcK src;                     // MODE 4: the motion source that replaces the random motion (riab_run_src)
 };
 
 // ---------------------------------------------------------------------------
@@ -134,6 +138,28 @@ __device__ __forceinline__ void agent_update_one(const riab_agents& ag, const ri
   store_agent(ag, i, s);
   if (io.pos_mirror != nullptr) *reinterpret_cast<double2*>(io.pos_mirror + 2 * (size_t)i) = make_double2(s.px, s.py);
   if (io.history_row != nullptr) store_history_row(io.history_row + 8 * (size_t)i, s);
+}
+
+// One agent's imported / forced Agent.update at time t (step io.step; same zero-displacement keys as the random branch).
+__device__ __forceinline__ void agent_update_src_one(const riab_agents& ag, const riab_motion_params& mp,
+                                                     const MotionDerived& md, const riab_step_io& io, const SrcK& src,
+                                                     double t, const EnvK& env, long long i, AgentState& s) {
+  load_agent(ag, i, s);
+  const unsigned long long gid = (unsigned long long)(ag.id_offset + i);
+  const double f1 = __longlong_as_double((long long)io.seed), f2 = __longlong_as_double((long long)(io.step ^ (gid << 20)));
+  source_step(s, src, i, t, mp, md, env.periodic != 0, env.scale, f1, f2);
+  store_agent(ag, i, s);
+  if (io.pos_mirror != nullptr) *reinterpret_cast<double2*>(io.pos_mirror + 2 * (size_t)i) = make_double2(s.px, s.py);
+  if (io.history_row != nullptr) store_history_row(io.history_row + 8 * (size_t)i, s);
+}
+
+__global__ void __launch_bounds__(128) k_agent_update_src(const riab_agents ag, const riab_motion_params mp,
+                                                          const MotionDerived md, const riab_step_io io, const SrcK src,
+                                                          const EnvK env) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ag.n_agents) return;
+  AgentState s;
+  agent_update_src_one(ag, mp, md, io, src, src.t, env, i, s);
 }
 
 template <bool REC>
@@ -870,8 +896,8 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
   if (warp >= RW) {
     // ------------------------------------------------------------- producers
     reg_set<C::REGS_PRODUCER, C::REGS_LAUNCH>();
-    if constexpr (MODE == 3) {
-      // whole run: this warp advances ITS tiles (q = pw, pw + MW, ...) step after step -- the same warp for every step of a
+    if constexpr (MODE >= 3) {
+      // whole run (MODE 4: following run.src instead of the random motion): this warp advances ITS tiles (q = pw, pw + MW, ...) step after step -- the same warp for every step of a
       // tile, so a tile's steps are ordered -- and publishes each (step, tile) record into its private ring (slots
       // pw + MW * i): the n-th record it produces goes to slot i = n % NSP in phase n / NSP
       constexpr int NSP = NS / MW;
@@ -879,6 +905,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
       // those steps must have other rows: riab_run launches whole runs with spikes only for ring_rows >= 2 >= NSP
       static_assert(NSP <= 2, "riab_run launches whole runs with spike rings of 2 rows");
       long long n = 0;
+      double t_st = run.src.t;                           // MODE 4: Agent.t of step st, advanced by `t += dt` like the host's
       for (long long st = 0; st < run.n_steps; ++st) {
         riab_step_io io_st = io;
         io_st.step = io.step + (unsigned long long)st;
@@ -893,12 +920,14 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
           bool nanpos = false;
           if (lane < na) {
             AgentState as;
-            agent_update_one<false>(ag, mp, md, io_st, env, s_walls, a0 + lane, as);
+            if constexpr (MODE == 4) agent_update_src_one(ag, mp, md, io_st, run.src, t_st, env, a0 + lane, as);
+            else agent_update_one<false>(ag, mp, md, io_st, env, s_walls, a0 + lane, as);
             nanpos = (as.px != as.px);
             P::record(s_slot[s].rec[lane], as.px, as.py, as.hdx, as.hdy, s_walls, s_aux, pc, env);
           }
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
         }
+        if constexpr (MODE == 4) t_st = t_st + mp.dt;
       }
     } else {
       for (long long q = pw; q < nq; q += MW) {
@@ -955,13 +984,13 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
     const int ex = P::expanded(pc);
     if constexpr (!NOISE) {
       if (lean) {
-        if (ex == 2) consumer_fast<P, SPK, C, 2, MODE == 3>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
-        else if (ex == 1) consumer_fast<P, SPK, C, 1, MODE == 3>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
-        else consumer_fast<P, SPK, C, 0, MODE == 3>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
+        if (ex == 2) consumer_fast<P, SPK, C, 2, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
+        else if (ex == 1) consumer_fast<P, SPK, C, 1, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
+        else consumer_fast<P, SPK, C, 0, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
         return;
       }
     }
-    if constexpr (MODE == 3) return;                    // (the host launches whole runs only where the lean loop applies)
+    if constexpr (MODE >= 3) return;                    // (the host launches whole runs only where the lean loop applies)
     if (ex == 2) consumer_slots<P, SPK, NOISE, C, 2>(pc, out, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
     else if (ex == 1) consumer_slots<P, SPK, NOISE, C, 1>(pc, out, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
     else consumer_slots<P, SPK, NOISE, C, 0>(pc, out, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
@@ -1598,7 +1627,8 @@ int make_ovc(const riab_ovc_cells* oc, const EnvK& env, const double* head_dir, 
 int g_num_sms = 0;
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
-// positions, then motion for the NEXT step -- used inside riab_run).
+// positions, then motion for the NEXT step -- used inside riab_run); 3: the whole run (RunK); 4: the whole run following
+// the motion source run->src.
 template <class P, int MODE>
 int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
                 const typename P::Const& pc, const OutK& out_in, const double* pos_in, long long n_rows, cudaStream_t s,
@@ -1936,6 +1966,71 @@ int riab_agent_update(const riab_agents* agents, const riab_env* env, const riab
   derive_motion(*prm, md);
   if (rec) k_agent_update<true><<<grid, 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
   else k_agent_update<false><<<grid, 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------- imported / forced motion
+int riab_trajectory_build(const riab_trajectory* tr, const double* times_host, void* stream) {
+  if (tr == nullptr || times_host == nullptr || tr->times_dev == nullptr || tr->y_dev == nullptr || tr->M_dev == nullptr)
+    return fail(RIAB_ERR_INVALID, "riab_trajectory_build: NULL argument");
+  const long long T = tr->T, ncol = 2 * tr->n_traj;
+  if (T < 4 || tr->n_traj <= 0) return fail(RIAB_ERR_INVALID, "riab_trajectory_build: T = %lld (>= 4 samples), n_traj = %lld", T, (long long)tr->n_traj);
+  for (long long i = 0; i + 1 < T; ++i)
+    if (!(times_host[i + 1] > times_host[i])) return fail(RIAB_ERR_INVALID, "riab_trajectory_build: times not strictly increasing at %lld", i);
+  std::vector<double> fac((size_t)(4 * (T - 2) + T - 1));
+  traj_factors(times_host, T, fac.data());
+  cudaStream_t s = (cudaStream_t)stream;
+  double* fac_dev = nullptr;
+  RIAB_CUDA_OK(cudaMallocAsync((void**)&fac_dev, fac.size() * sizeof(double), s));
+  RIAB_CUDA_OK(cudaMemcpyAsync(fac_dev, fac.data(), fac.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  k_traj_build<<<(unsigned)((ncol + 127) / 128), 128, 0, s>>>(tr->y_dev, tr->M_dev, fac_dev, T, ncol);
+  g_launches++;
+  const cudaError_t e = cudaGetLastError();
+  RIAB_CUDA_OK(cudaFreeAsync(fac_dev, s));
+  // the pageable source of the copy must outlive it
+  RIAB_CUDA_OK(cudaStreamSynchronize(s));
+  if (e != cudaSuccess) return fail(RIAB_ERR_CUDA, "k_traj_build: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+}  // extern "C"
+static int make_src(const riab_motion_source* src, long long n_agents, SrcK& k) {
+  memset(&k, 0, sizeof(k));
+  k.kind = src->kind;
+  k.t = src->t;
+  if (src->kind == RIAB_MOTION_IMPORTED) {
+    const riab_trajectory& tr = src->traj;
+    if (tr.times_dev == nullptr || tr.y_dev == nullptr || tr.M_dev == nullptr || tr.T < 4 || !(tr.t_max > 0.0))
+      return fail(RIAB_ERR_INVALID, "motion source: bad trajectory");
+    if (tr.n_traj != 1 && tr.n_traj != n_agents)
+      return fail(RIAB_ERR_INVALID, "motion source: %lld trajectories for %lld agents", (long long)tr.n_traj, n_agents);
+    k.times = tr.times_dev; k.y = tr.y_dev; k.M = tr.M_dev; k.T = tr.T; k.n_traj = tr.n_traj; k.t_max = tr.t_max;
+    return 0;
+  }
+  if (src->kind == RIAB_MOTION_FORCED) {
+    if (src->forced_dev == nullptr) return fail(RIAB_ERR_INVALID, "motion source: forced positions NULL");
+    k.forced = src->forced_dev; k.bcast = src->forced_broadcast != 0;
+    return 0;
+  }
+  return fail(RIAB_ERR_INVALID, "motion source: kind %d", src->kind);
+}
+extern "C" {
+
+int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
+                          const riab_step_io* io, const riab_motion_source* src, void* stream) {
+  if (src == nullptr || src->kind == RIAB_MOTION_RANDOM) return riab_agent_update(agents, env, prm, io, stream);
+  EnvK ek;
+  SrcK sk;
+  int rc;
+  if ((rc = check_agents(agents)) || (rc = make_env(env, ek)) || (rc = check_motion(prm))) return rc;
+  if (io == nullptr) return fail(RIAB_ERR_INVALID, "io is NULL");
+  if ((rc = make_src(src, agents->n_agents, sk))) return rc;
+  if (agents->n_agents == 0) return 0;
+  MotionDerived md;
+  derive_motion(*prm, md);
+  k_agent_update_src<<<(unsigned)((agents->n_agents + 127) / 128), 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, sk, ek);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;
@@ -2375,9 +2470,11 @@ int riab_neurons_update(const riab_agents* agents, const riab_env* env, int32_t 
   return neurons_update_impl<0>(agents, env, nullptr, nullptr, cells_kind, cells, noise, out, stream);
 }
 
-int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
-             const riab_population* pops, int32_t n_pops, const riab_agent_history* hist, int64_t n_steps,
-             void* stream) {
+}  // extern "C"
+// riab_run / riab_run_src.  src: NULL for the random motion, else an imported trajectory (already checked).
+static int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
+                    const riab_motion_source* src, const riab_population* pops, int32_t n_pops,
+                    const riab_agent_history* hist, int64_t n_steps, void* stream) {
   if (agents == nullptr || io == nullptr || n_pops < 0 || (n_pops > 0 && pops == nullptr))
     return fail(RIAB_ERR_INVALID, "riab_run: bad argument");
   const int64_t A = agents->n_agents;
@@ -2392,7 +2489,18 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
   bool any_ffl = false;
   for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
   const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && !any_ffl && n_steps >= 1 &&
-                    io->xi == nullptr && !io->collision_mask && !io->first_hit && !io->n_iters;
+                    io->xi == nullptr && !io->collision_mask && !io->first_hit && !io->n_iters && src == nullptr;
+  // a motion source keeps the plain schedule (its motion kernel is cheap next to the rates): per step, the motion kernel
+  // of the step and then every population, except for the whole-run case below.  Step st's clock: t_st = t_{st-1} + dt
+  riab_motion_source src_st;
+  if (src != nullptr) src_st = *src;
+  auto motion = [&](const riab_step_io& sio) {
+    if (src == nullptr) return riab_agent_update(agents, env, prm, &sio, stream);
+    const int r = riab_agent_update_src(agents, env, prm, &sio, &src_st, stream);
+    src_st.t = src_st.t + prm->dt;
+    return r;
+  };
+  const bool whole = src == nullptr ? skew : (n_pops >= 1 && n_steps >= 1 && !any_ffl);
   auto step_io = [&](int64_t st) {
     riab_step_io sio = *io;
     sio.step = io->step + (uint64_t)st;
@@ -2409,7 +2517,7 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
   // soon as its private ring (at most 2 records) has room, while the consumers may still RED.OR step s's thinned spikes;
   // with ring_rows >= 2 those are different rows, with one row nothing orders the clear after the ORs, so that case takes
   // the per-step loop (stream-ordered launches)
-  if (n_pops == 1 && skew && getenv("RIAB_NO_WHOLE_RUN") == nullptr && io->drift_velocity == nullptr && io->pos_mirror == nullptr) {
+  if (n_pops == 1 && whole && getenv("RIAB_NO_WHOLE_RUN") == nullptr && io->drift_velocity == nullptr && io->pos_mirror == nullptr) {
     const riab_population& pp = pops[0];
     EnvK ek;
     OutK ok;
@@ -2456,6 +2564,11 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
         riab_step_io io0 = *io;
         io0.history_row = nullptr;
         cudaStream_t s = (cudaStream_t)stream;
+        if (src != nullptr) {
+          if ((rc = make_src(src, A, run.src))) return rc;
+          if (place) return launch_place<4>(ek, *agents, *prm, io0, pcst, ok, nullptr, A, s, &run);
+          return launch_tile<GridPolicy, 4>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
+        }
         if (place) return launch_place<3>(ek, *agents, *prm, io0, pcst, ok, nullptr, A, s, &run);
         return launch_tile<GridPolicy, 3>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
       }
@@ -2521,13 +2634,13 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
   for (int64_t st = 0; st < n_steps; ++st) {
     if (pipe) pipe->step = st;
     const riab_step_io sio = step_io(st);
-    if (n_pops == 0) {
-      if ((rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
-      continue;
+    if (n_pops == 0 || src != nullptr) {
+      if ((rc = motion(sio))) return rc;
+      if (n_pops == 0) continue;
     }
     // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
     // FeedForwardLayers in registration order, after every row they read of this step exists
-    if (!skew && pops[0].kind == RIAB_CELLS_FFL && (rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
+    if (!skew && src == nullptr && pops[0].kind == RIAB_CELLS_FFL && (rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
     for (int pi = 0; pi < 2 * n_pops; ++pi) {
       const int p = pi >= n_pops ? pi - n_pops : (skew ? ((pi + 1) % n_pops) : pi);
       const riab_population& pp = pops[p];
@@ -2563,7 +2676,8 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
           in.ld = ip.out.ld;
         }
         rc = riab_neurons_update(agents, env, pp.kind, &fc, &nz, &ro, stream);
-      } else if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
+      } else if (p == 0 && src != nullptr) rc = riab_neurons_update(agents, env, pp.kind, pp.cells, &nz, &ro, stream);
+      else if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
       else if (p == 0 && st + 1 < n_steps) {
         const riab_step_io nxt = step_io(st + 1);          // the motion it runs belongs to step st+1
         rc = neurons_update_impl<2>(agents, env, prm, &nxt, pp.kind, pp.cells, &nz, &ro, stream);
@@ -2572,6 +2686,26 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
     }
   }
   return 0;
+}
+
+extern "C" {
+
+int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
+             const riab_population* pops, int32_t n_pops, const riab_agent_history* hist, int64_t n_steps,
+             void* stream) {
+  return run_impl(agents, env, prm, io, nullptr, pops, n_pops, hist, n_steps, stream);
+}
+
+int riab_run_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
+                 const riab_motion_source* src, const riab_population* pops, int32_t n_pops,
+                 const riab_agent_history* hist, int64_t n_steps, void* stream) {
+  if (src == nullptr || src->kind == RIAB_MOTION_RANDOM) return riab_run(agents, env, prm, io, pops, n_pops, hist, n_steps, stream);
+  if (src->kind != RIAB_MOTION_IMPORTED) return fail(RIAB_ERR_UNSUPPORTED, "riab_run_src: a forced position belongs to one step");
+  if (agents == nullptr) return fail(RIAB_ERR_INVALID, "riab_run: bad argument");
+  SrcK sk;
+  int rc;
+  if ((rc = make_src(src, agents->n_agents, sk))) return rc;
+  return run_impl(agents, env, prm, io, src, pops, n_pops, hist, n_steps, stream);
 }
 
 int riab_step_fused_host(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,

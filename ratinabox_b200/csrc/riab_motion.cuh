@@ -110,6 +110,66 @@ RIAB_DEV bool env_contains(double x, double y, const double* __restrict__ walls,
   return (n_hole == 0) || !edges_contain(x, y, walls + 4 * hole0, n_hole);
 }
 
+// A pos / prev_pos pair's displacement; through the boundary when periodic (Environment.py:670-675)
+RIAB_DEV void step_displacement(D px, D py, D ppx, D ppy, bool periodic, double scale, D& stx, D& sty) {
+  stx = px - ppx; sty = py - ppy;
+  if (periodic) {
+    const double half = scale / 2;
+    if (fabs(stx.v) > half) stx = D(-copysign(1.0, stx.v)) * (D(scale) - D(fabs(stx.v)));
+    if (fabs(sty.v) > half) sty = D(-copysign(1.0, sty.v)) * (D(scale) - D(fabs(sty.v)));
+  }
+}
+
+// A8-A10 of Agent.update, after the position of the step is known: measured velocity / rotational velocity, head
+// direction and distance travelled from the step's displacement (stx, sty) and the previous measured velocity.
+// Writes s.mrot, s.hdx, s.hdy, s.dist and returns the measured velocity in (mvx, mvy); the caller stores it.  SOURCE:
+// the imported / forced branches (_measure_velocity_of_step_taken(overwrite_velocity=True), Agent.py:444-472): a NaN
+// in pos or prev_pos (nan_step) makes the measured velocities NaN and adds 0 to the distance travelled.
+template <bool SOURCE>
+RIAB_DEV void measure_tail(AgentState& s, D stx, D sty, double pmvx, double pmvy, D dt, const riab_motion_params& p,
+                           const MotionDerived& m, double fallback_n1, double fallback_n2, D& mvx, D& mvy,
+                           bool nan_step = false) {
+  // ---- A8: measured velocity / rotational velocity (Agent.py:444-472)
+  mvx = stx / dt; mvy = sty / dt;
+  if (SOURCE && nan_step) { mvx = D(__longlong_as_double(0x7ff8000000000000ll)); mvy = mvx; }     // Agent.py:451-454
+  if (dsqrt(mvx * mvx + mvy * mvy).v == 0.0) {
+    // 1e-8 * randn(2) in the reference; here a Philox draw keyed by the (bit-cast) seed / step^agent words
+    uint32_t c[4] = {(uint32_t)__double_as_longlong(fallback_n2), (uint32_t)(__double_as_longlong(fallback_n2) >> 32),
+                     0x4d454153u, RIAB_STREAM_MEASURE << 24};
+    philox4x32_10(c, (uint32_t)__double_as_longlong(fallback_n1), (uint32_t)(__double_as_longlong(fallback_n1) >> 32));
+    mvx = D(1e-8 * (2.0 * u01_53(c[0], c[1]) - 1.0));
+    mvy = D(1e-8 * (2.0 * u01_53(c[2], c[3]) - 1.0));
+  }
+  {
+    // utils.pi_domain(get_angle(now) - get_angle(before)) (utils.py:231-273, :331-341).  get_angle is
+    // atan2(y, x + 1e-6) mod 2pi; the wrapped difference of the two angles equals the signed angle
+    // between the eps-shifted vectors, atan2(cross, dot): one atan2 instead of two plus three fmods
+    // (identical up to rounding; pi_domain maps to (-pi, pi] like atan2).
+    const double x1 = __dadd_rn(pmvx, 1e-6), y1 = pmvy, x2 = __dadd_rn(mvx.v, 1e-6), y2 = mvy.v;
+    const double ang = atan2(x1 * y2 - y1 * x2, x1 * x2 + y1 * y2);
+    s.mrot = __ddiv_rn(ang, dt.v);
+  }
+
+  // ---- A9: head direction low-pass (Agent.py:474-500)
+  {
+    const D nmv = dsqrt(mvx * mvx + mvy * mvy);
+    const D ix = mvx / nmv, iy = mvy / nmv;
+    const D tau(p.head_direction_smoothing_timescale);
+    if (tau.v <= dt.v) { s.hdx = ix.v; s.hdy = iy.v; }
+    else {
+      const D a(m.hd_a), b(m.hd_b);
+      const D hx = D(s.hdx) * a + b * ix, hy = D(s.hdy) * a + b * iy;
+      const D nh = dsqrt(hx * hx + hy * hy);
+      s.hdx = (hx / nh).v; s.hdy = (hy / nh).v;
+    }
+  }
+
+  // ---- A10: distance travelled (Agent.py:502-507; a NaN in pos or prev_pos adds 0)
+  if (!SOURCE || !nan_step) {
+    s.dist = (D(s.dist) + dsqrt(stx * stx + sty * sty)).v;
+  }
+}
+
 // walls: shared/global array of W*(ax,ay,bx,by) doubles.
 // REC: write the per-iteration collision masks (parity taps).
 template <bool REC>
@@ -258,52 +318,9 @@ RIAB_DEV void motion_step(AgentState& s, const double* __restrict__ walls, int W
       py = D(fmin(fmax(py.v, ext[2] + 0.01), ext[3] - 0.01));
     }
   }
-  // displacement of the step; through the boundary when periodic (Environment.py:670-675)
-  D stx = px - ppx, sty = py - ppy;
-  if (periodic) {
-    const double half = scale / 2;
-    if (fabs(stx.v) > half) stx = D(-copysign(1.0, stx.v)) * (D(scale) - D(fabs(stx.v)));
-    if (fabs(sty.v) > half) sty = D(-copysign(1.0, sty.v)) * (D(scale) - D(fabs(sty.v)));
-  }
-
-  // ---- A8: measured velocity / rotational velocity (Agent.py:444-472)
-  D mvx = stx / dt, mvy = sty / dt;
-  if (dsqrt(mvx * mvx + mvy * mvy).v == 0.0) {
-    // 1e-8 * randn(2) in the reference; here a Philox draw keyed by the (bit-cast) seed / step^agent words
-    uint32_t c[4] = {(uint32_t)__double_as_longlong(fallback_n2), (uint32_t)(__double_as_longlong(fallback_n2) >> 32),
-                     0x4d454153u, RIAB_STREAM_MEASURE << 24};
-    philox4x32_10(c, (uint32_t)__double_as_longlong(fallback_n1), (uint32_t)(__double_as_longlong(fallback_n1) >> 32));
-    mvx = D(1e-8 * (2.0 * u01_53(c[0], c[1]) - 1.0));
-    mvy = D(1e-8 * (2.0 * u01_53(c[2], c[3]) - 1.0));
-  }
-  {
-    // utils.pi_domain(get_angle(now) - get_angle(before)) (utils.py:231-273, :331-341).  get_angle is
-    // atan2(y, x + 1e-6) mod 2pi; the wrapped difference of the two angles equals the signed angle
-    // between the eps-shifted vectors, atan2(cross, dot): one atan2 instead of two plus three fmods
-    // (identical up to rounding; pi_domain maps to (-pi, pi] like atan2).
-    const double x1 = __dadd_rn(pmvx, 1e-6), y1 = pmvy, x2 = __dadd_rn(mvx.v, 1e-6), y2 = mvy.v;
-    const double ang = atan2(x1 * y2 - y1 * x2, x1 * x2 + y1 * y2);
-    s.mrot = __ddiv_rn(ang, dt.v);
-  }
-
-  // ---- A9: head direction low-pass (Agent.py:474-500)
-  {
-    const D nmv = dsqrt(mvx * mvx + mvy * mvy);
-    const D ix = mvx / nmv, iy = mvy / nmv;
-    const D tau(p.head_direction_smoothing_timescale);
-    if (tau.v <= dt.v) { s.hdx = ix.v; s.hdy = iy.v; }
-    else {
-      const D a(m.hd_a), b(m.hd_b);
-      const D hx = D(s.hdx) * a + b * ix, hy = D(s.hdy) * a + b * iy;
-      const D nh = dsqrt(hx * hx + hy * hy);
-      s.hdx = (hx / nh).v; s.hdy = (hy / nh).v;
-    }
-  }
-
-  // ---- A10: distance travelled (Agent.py:502-507)
-  {
-    s.dist = (D(s.dist) + dsqrt(stx * stx + sty * sty)).v;
-  }
+  D stx, sty, mvx, mvy;
+  step_displacement(px, py, ppx, ppy, periodic, scale, stx, sty);
+  measure_tail<false>(s, stx, sty, pmvx, pmvy, dt, p, m, fallback_n1, fallback_n2, mvx, mvy);
   s.px = px.v; s.py = py.v; s.vx = vx.v; s.vy = vy.v; s.rot = rot.v; s.mvx = mvx.v; s.mvy = mvy.v;
 }
 
