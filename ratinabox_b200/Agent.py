@@ -227,9 +227,7 @@ class Agent:
             # stream + one stream sync.  `Ag.pos` hands out a fresh COPY of it (reference-style code keeps
             # such arrays: `traj.append(Ag.pos)`); in-place edits of that copy are not tracked -- assign to
             # write (``Ag.pos = new_positions``).  state_view() returns the staging buffer itself.
-            buf = self._pinned.get(name)
-            if buf is None:
-                buf = self._pinned[name] = torch.empty(t.shape, dtype=t.dtype).pin_memory()
+            buf = self._pinned_buffer(name)
             if name == "pos" and self._pos_mirror_current and self._motion_event_valid:
                 # the copy engine is bringing the positions into this buffer: wait for that copy only
                 _lib.check(self._lib.riab_positions_wait())
@@ -250,6 +248,16 @@ class Agent:
         if isinstance(val, np.ndarray):
             self._shadow[name] = (val, val.copy())
         return val
+
+    def _pinned_buffer(self, name):
+        """The page-locked host copy of a state array that large batches read through (the motion kernels post the
+        positions straight into the "pos" one)."""
+        buf = self._pinned.get(name)
+        if buf is None:
+            import torch
+            t = self._s[name]
+            buf = self._pinned[name] = torch.empty(t.shape, dtype=t.dtype).pin_memory()
+        return buf
 
     def state_view(self, name="pos"):
         """Zero-copy, READ-ONLY view of a state array in page-locked host memory, shape (n_agents, ...) -- the opt-in
@@ -417,29 +425,8 @@ class Agent:
         forced = kwargs.get("forced_next_position", None)
         if self.use_imported_trajectory or forced is not None:
             return self._update_source(dt, forced, kwargs)
-        dt = (dt or self.dt)
-        self.dt = dt
-        self.prev_t = self.t
-        self.t += dt
         self._sync_user_writes()
-
-        mp = self._mp
-        mp.dt = float(dt)
-        mp.speed_coherence_time_kw = float(kwargs.get("speed_coherence_time", self.speed_coherence_time))
-        mp.speed_mean_kw = float(kwargs.get("speed_mean", self.speed_mean))
-        mp.speed_mean = float(self.speed_mean)
-        mp.speed_std = float(self.speed_std)
-        mp.speed_coherence_time = float(self.speed_coherence_time)
-        mp.rotational_velocity_coherence_time_kw = float(
-            kwargs.get("rotational_velocity_coherence_time", self.rotational_velocity_coherence_time))
-        mp.rotational_velocity_std_kw = float(kwargs.get("rotational_velocity_std", self.rotational_velocity_std))
-        mp.rotational_velocity_drift_kw = float(kwargs.get("rotational_velocity_drift", 0))
-        mp.head_direction_smoothing_timescale = float(self.head_direction_smoothing_timescale)
-        mp.thigmotaxis_kw = float(kwargs.get("thigmotaxis", self.thigmotaxis))
-        mp.wall_repel_distance_kw = float(kwargs.get("wall_repel_distance", self.wall_repel_distance))
-        mp.wall_repel_strength_kw = float(kwargs.get("wall_repel_strength", self.wall_repel_strength))
-        mp.drift_to_random_strength_ratio = float(drift_to_random_strength_ratio)
-
+        self._fill_motion_params(dt or self.dt, kwargs, drift_to_random_strength_ratio)
         io = self._io
         io.drift_velocity = None
         self._drift_host_ptr = None
@@ -477,8 +464,6 @@ class Agent:
             self._tape = torch.as_tensor(np.ascontiguousarray(xi, dtype=np.float64).reshape(self.n_agents, 2),
                                          device=self.device)
             io.xi = self._tape.data_ptr()
-        io.seed = int(self.seed) & 0xFFFFFFFFFFFFFFFF
-        io.step = self._step
         io.collision_mask = io.first_hit = io.n_iters = None
         self._rec = None
         if kwargs.get("_record_collisions", False):
@@ -490,21 +475,14 @@ class Agent:
             io.collision_mask = self._rec["mask"].data_ptr()
             io.first_hit = self._rec["first_hit"].data_ptr()
             io.n_iters = self._rec["n_iters"].data_ptr()
-        io.history_row = None
-        if self.save_history:
-            io.history_row = self._history_row_ptr()
-            self._t_hist.append(self.t)
+        self._stage_step(dt)
         io.pos_mirror = None
         if self.n_agents > self._SHADOW_MAX and (self.fused_step or self._staging_only):
             # large batches: the motion step also posts the new positions into the pinned host buffer that
             # `Ag.pos` hands out, so reading them back after the step costs a stream sync and no copy
-            buf = self._pinned.get("pos")
-            if buf is None:
-                buf = self._pinned["pos"] = torch.empty((self.n_agents, 2), dtype=torch.float64).pin_memory()
-            io.pos_mirror = buf.data_ptr()
+            io.pos_mirror = self._pinned_buffer("pos").data_ptr()
             self._pos_mirror_current = True
         self._pending = True
-        self._step += 1
         if not self.fused_step and not self._staging_only:
             self._flush_pending()                      # launch the motion kernel now (asynchronous)
 
@@ -526,34 +504,40 @@ class Agent:
         mp.wall_repel_strength_kw = float(kwargs.get("wall_repel_strength", self.wall_repel_strength))
         mp.drift_to_random_strength_ratio = float(drift_to_random_strength_ratio)
 
-    def _update_source(self, dt, forced, kwargs):
-        """The imported / forced branches of Agent.update (Agent.py:219-242).  The motion kernel is launched at once
-        (with fused_step too: the rates then take the unfused path), except while run() stages its first step."""
-        if not self.use_imported_trajectory:
-            self._stage_source(forced)          # validates before the clock moves
+    def _stage_step(self, dt):
+        """The clock (t += dt, like the reference's), the Philox key and the agent-history row of the step that
+        update() stages."""
         dt = (dt or self.dt)
         self.dt = dt
         self.prev_t = self.t
         self.t += dt
-        self._sync_user_writes()
-        if self.use_imported_trajectory:
-            self._stage_source(None)
-        self._fill_motion_params(dt, kwargs)
         io = self._io
-        io.drift_velocity = io.xi = None
-        io.collision_mask = io.first_hit = io.n_iters = None
-        io.pos_mirror = None
-        self._tape = self._rec = None
-        self._drift_host_ptr = None
         io.seed = int(self.seed) & 0xFFFFFFFFFFFFFFFF
         io.step = self._step
         io.history_row = None
         if self.save_history:
             io.history_row = self._history_row_ptr()
             self._t_hist.append(self.t)
+        self._step += 1
+        return io
+
+    def _update_source(self, dt, forced, kwargs):
+        """The imported / forced branches of Agent.update (Agent.py:219-242).  The motion kernel is launched at once
+        (with fused_step too: the rates then take the unfused path), except while run() stages its first step."""
+        if not self.use_imported_trajectory:
+            self._stage_source(forced)          # validates before the clock moves
+        self._sync_user_writes()
+        io = self._stage_step(dt)
+        if self.use_imported_trajectory:
+            self._stage_source(None)
+        self._fill_motion_params(self.dt, kwargs)
+        io.drift_velocity = io.xi = None
+        io.collision_mask = io.first_hit = io.n_iters = None
+        io.pos_mirror = None
+        self._tape = self._rec = None
+        self._drift_host_ptr = None
         self._pos_mirror_current = False
         self._motion_event_valid = False
-        self._step += 1
         if self._staging_only:
             return
         self._wait_pos_copy()
@@ -580,11 +564,7 @@ class Agent:
             # then wait for that download only, not for the rate kernels queued behind the motion kernel
             pos_out = None
             if self.n_agents > self._SHADOW_MAX:
-                import torch
-                buf = self._pinned.get("pos")
-                if buf is None:
-                    buf = self._pinned["pos"] = torch.empty((self.n_agents, 2), dtype=torch.float64).pin_memory()
-                pos_out = buf.data_ptr()
+                pos_out = self._pinned_buffer("pos").data_ptr()
             stage = self._drift_dev.data_ptr() if self._drift_host_ptr is not None else None
             _lib.check(self._lib.riab_agent_update_host(C.byref(self._agents_c), C.byref(self._env_struct()), C.byref(self._mp),
                                                         C.byref(self._io), self._drift_host_ptr, stage, pos_out, self._stream()))

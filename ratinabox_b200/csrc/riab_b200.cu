@@ -8,7 +8,7 @@
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
-//   k_bvc_rays<FUSED>   BVC phase A (float64 rays) [+ Agent.update]
+//   k_bvc_rays<TABLE>   BVC phase A (float64 rays)
 //   k_bvc_integrate     BVC phase B (float32 angular integral, TMA-staged tables)
 #include <algorithm>
 #include <atomic>
@@ -1118,10 +1118,9 @@ __global__ void __launch_bounds__(NT) k_finish_rows(const OutK out, const int n_
 }
 
 // ---------------------------------------------------------------------------
-// BVC phase A (+ optional fused Agent.update): one CTA per tile of 32 agents.
-template <bool FUSED, bool REC, bool TABLE>
-__global__ void __launch_bounds__(NT, (TABLE && !FUSED) ? 4 : 1) k_bvc_rays(const EnvK env, const riab_agents ag, const riab_motion_params mp,
-                                                 const MotionDerived md, const riab_step_io io, const BvcConst bc,
+// BVC phase A: one CTA per tile of 32 agents.
+template <bool TABLE>
+__global__ void __launch_bounds__(NT, TABLE ? 4 : 1) k_bvc_rays(const EnvK env, const BvcConst bc,
                                                  const double* __restrict__ pos_in, const long long n_rows,
                                                  float* __restrict__ scratch, int32_t* __restrict__ first_wall,
                                                  uint32_t* __restrict__ spikes_zero, const long long spike_ld) {
@@ -1143,13 +1142,7 @@ __global__ void __launch_bounds__(NT, (TABLE && !FUSED) ? 4 : 1) k_bvc_rays(cons
     double px = 0.5 * (env.ext[0] + env.ext[1]), py = 0.5 * (env.ext[2] + env.ext[3]);   // padding rows: box centre
     if ((int)threadIdx.x < na) {
       const long long i = a0 + threadIdx.x;
-      if (FUSED) {
-        AgentState s;
-        agent_update_one<REC>(ag, mp, md, io, env, s_walls, i, s);
-        px = s.px; py = s.py;
-      } else {
-        px = pos_in[2 * i]; py = pos_in[2 * i + 1];
-      }
+      px = pos_in[2 * i]; py = pos_in[2 * i + 1];
     }
     s_pos[threadIdx.x][0] = px;
     s_pos[threadIdx.x][1] = py;
@@ -1747,16 +1740,24 @@ struct BvcPipe {
   float* scratch2[PIPE_POPS] = {};
   long long step = 0;
 };
-thread_local BvcPipe* g_pipe = nullptr;
 
-template <bool FUSED>
-int launch_bvc(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
-               const riab_bvc_cells* bvc, const OutK& out, const double* pos_in, long long n_rows, float* scratch,
-               int32_t* first_wall, const double* head_dir, cudaStream_t s) {
+int check_bvc(const EnvK& env, const riab_bvc_cells* bvc, const float* scratch, long long n_rows) {
   if (bvc == nullptr || bvc->packed_dev == nullptr || bvc->test_dirs_dev == nullptr)
     return fail(RIAB_ERR_INVALID, "bvc cells / packed_dev / test_dirs_dev NULL");
   if (scratch == nullptr) return fail(RIAB_ERR_INVALID, "bvc scratch NULL");
   if (env.periodic) return fail(RIAB_ERR_INVALID, "boundary cells only possible with solid boundary conditions (Neurons.py:1580-1582)");
+  if (n_rows == 0) return 0;
+  const int T = bvc->n_test_angles;
+  if ((size_t)T * (BVC_CT + 2 * BVC_AT) * sizeof(float) > 220 * 1024)
+    return fail(RIAB_ERR_UNSUPPORTED, "n_test_angles=%d too large for shared memory", T);
+  if ((T * BVC_AT * 4) % 16 != 0 || ((uintptr_t)scratch) % 16 != 0 || ((uintptr_t)bvc->packed_dev) % 16 != 0)
+    return fail(RIAB_ERR_INVALID, "bvc buffers must be 16-byte aligned");
+  return 0;
+}
+
+// One BVC evaluation over n_rows rows, checked by check_bvc.  pipe: riab_run's pipeline, or NULL.
+int launch_bvc(const EnvK& env, const riab_bvc_cells* bvc, const OutK& out, const double* pos_in, long long n_rows,
+               float* scratch, int32_t* first_wall, const double* head_dir, cudaStream_t s, BvcPipe* pipe = nullptr) {
   if (n_rows == 0) return 0;
   BvcConst bc;
   bc.n_cells = bvc->n_cells; bc.n_pad = bvc->n_pad; bc.T = bvc->n_test_angles;
@@ -1766,18 +1767,11 @@ int launch_bvc(const EnvK& env, const riab_agents& ag, const riab_motion_params&
   const long long n_tiles = (n_rows + BVC_AT - 1) / BVC_AT;
   const size_t smemA = (size_t)bc.T * 2 * sizeof(double);
   const size_t smemB = (size_t)bc.T * (BVC_CT + 2 * BVC_AT) * sizeof(float);
-  if (smemB > 220 * 1024) return fail(RIAB_ERR_UNSUPPORTED, "n_test_angles=%d too large for shared memory", bc.T);
-  if ((bc.T * BVC_AT * 4) % 16 != 0 || ((uintptr_t)scratch) % 16 != 0 || ((uintptr_t)bvc->packed_dev) % 16 != 0)
-    return fail(RIAB_ERR_INVALID, "bvc buffers must be 16-byte aligned");
-  const bool rec = FUSED && (io.collision_mask || io.first_hit || io.n_iters);
-  MotionDerived md;
-  memset(&md, 0, sizeof(md));
-  if (FUSED) derive_motion(mp, md);
   // spikes without OU noise are drawn in the integration kernel's epilogue (the ray kernel clears the rows first);
   // OU noise (a read-modify-write of the noise state per rate) and odd shard offsets keep the k_finish_rows post-pass
   const int fold = (out.spikes != nullptr && out.noise == nullptr && (out.id_offset & 1ll) == 0) ? 1 : 0;
   uint32_t* const zsp = fold ? out.spikes : nullptr;
-  BvcPipe* const pipe = (g_pipe != nullptr && !bc.ego && out.pop >= 0 && out.pop < PIPE_POPS && g_pipe->scratch2[out.pop] != nullptr) ? g_pipe : nullptr;
+  if (pipe != nullptr && (out.pop < 0 || out.pop >= PIPE_POPS || pipe->scratch2[out.pop] == nullptr)) pipe = nullptr;
   const int pb = pipe ? (int)(pipe->step & 1) : 0;
   if (pipe) {
     if (pb) scratch = pipe->scratch2[out.pop];
@@ -1788,13 +1782,8 @@ int launch_bvc(const EnvK& env, const riab_agents& ag, const riab_motion_params&
   // two integration CTAs of the previous step, 2 x 92 KB at T = 180)
   const size_t smemT = smemA + (size_t)bc.T * (sizeof(float2) + (size_t)env.W * sizeof(BvcTab));
   const bool table = env.W <= BVC_NW && smemT <= 40 * 1024;
-  if (table) {
-    if (rec) k_bvc_rays<FUSED, FUSED, true><<<(unsigned)n_tiles, NT, smemT, s>>>(env, ag, mp, md, io, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
-    else k_bvc_rays<FUSED, false, true><<<(unsigned)n_tiles, NT, smemT, s>>>(env, ag, mp, md, io, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
-  } else {
-    if (rec) k_bvc_rays<FUSED, FUSED, false><<<(unsigned)n_tiles, NT, smemA, s>>>(env, ag, mp, md, io, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
-    else k_bvc_rays<FUSED, false, false><<<(unsigned)n_tiles, NT, smemA, s>>>(env, ag, mp, md, io, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
-  }
+  if (table) k_bvc_rays<true><<<(unsigned)n_tiles, NT, smemT, s>>>(env, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
+  else k_bvc_rays<false><<<(unsigned)n_tiles, NT, smemA, s>>>(env, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   if (pipe) {                                         // the integral (and its post-pass) go to the side stream
@@ -1848,7 +1837,6 @@ int ffl_tmap(CUtensorMap* map, const float* base, long long inner, long long out
     if (q != cudaDriverEntryPointSuccess || fn == nullptr) return fail(RIAB_ERR_CUDA, "cuTensorMapEncodeTiled not found");
     encode = (EncodeTiledFn)fn;
   }
-  if (((uintptr_t)base) % 16 != 0 || (ld * 4) % 16 != 0) return fail(RIAB_ERR_INVALID, "FFL operands need 16-byte aligned rows");
   const cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
   const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
   const cuuint32_t box[2] = {(cuuint32_t)FFL_BK, (cuuint32_t)box_outer};
@@ -1872,14 +1860,28 @@ int launch_ffl_bn(FflK& k, cudaStream_t s) {
   return 0;
 }
 
-// One FeedForwardLayer evaluation over n_rows rows (+ noise / spikes through the k_finish_rows post-pass).
-int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, const OutK& out, cudaStream_t s) {
+int check_ffl(const riab_ffl_cells* f, const OutK& out, long long n_rows) {
   if (f == nullptr || f->bias_dev == nullptr) return fail(RIAB_ERR_INVALID, "ffl / bias_dev NULL");
   if (f->n_cells <= 0) return fail(RIAB_ERR_INVALID, "ffl: n_cells must be > 0");
   if (f->n_inputs < 0 || f->n_inputs > RIAB_FFL_MAX_INPUTS)
     return fail(RIAB_ERR_UNSUPPORTED, "ffl: %d inputs (at most %d)", f->n_inputs, RIAB_FFL_MAX_INPUTS);
   if (f->activation < RIAB_ACT_LINEAR || f->activation > RIAB_ACT_SOFTPLUS) return fail(RIAB_ERR_INVALID, "ffl: bad activation %d", f->activation);
   if (f->prime_dev != nullptr && out.ld % 4 != 0) return fail(RIAB_ERR_INVALID, "ffl: ld must be a multiple of 4");
+  if (n_rows == 0) return 0;
+  for (int i = 0; i < f->n_inputs; ++i) {
+    const riab_ffl_input& in = f->inputs[i];
+    if (in.rows_dev == nullptr) continue;                        // an input that was never updated contributes zeros
+    if (in.w_dev == nullptr || in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || in.ld < in.n_in)
+      return fail(RIAB_ERR_INVALID, "ffl input %d: bad weights / sizes (pack with riab_ffl_pack)", i);
+    if (((uintptr_t)in.rows_dev) % 16 != 0 || (in.ld * 4) % 16 != 0 || ((uintptr_t)in.w_dev) % 16 != 0)
+      return fail(RIAB_ERR_INVALID, "FFL operands need 16-byte aligned rows");
+  }
+  return 0;
+}
+
+// One FeedForwardLayer evaluation over n_rows rows (+ noise / spikes through the k_finish_rows post-pass), checked by
+// check_ffl.
+int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, const OutK& out, cudaStream_t s) {
   if (n_rows == 0) return 0;
   // N tile: the wgmma N of 8, 32 or 64 that wastes least (64: accumulator + per-stage partial = 64 registers)
   const int bn = f->n_cells <= 8 ? 8 : (f->n_cells <= 32 ? 32 : 64);
@@ -1889,9 +1891,7 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
   const int n_pad = (f->n_cells + 7) / 8 * 8;
   for (int i = 0; i < f->n_inputs; ++i) {
     const riab_ffl_input& in = f->inputs[i];
-    if (in.rows_dev == nullptr) continue;                        // an input that was never updated contributes zeros
-    if (in.w_dev == nullptr || in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || in.ld < in.n_in)
-      return fail(RIAB_ERR_INVALID, "ffl input %d: bad weights / sizes (pack with riab_ffl_pack)", i);
+    if (in.rows_dev == nullptr) continue;
     const int l = k.n_inputs++;
     if ((rc = ffl_tmap(&k.in[l], in.rows_dev, in.n_in, n_rows, in.ld, FFL_BM)) ||
         (rc = ffl_tmap(&k.whi[l], in.w_dev, in.k_pad, n_pad, in.k_pad, bn)) ||
@@ -1915,10 +1915,400 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
   return 0;
 }
 
+
+int make_src(const riab_motion_source* src, long long n_agents, SrcK& k) {
+  memset(&k, 0, sizeof(k));
+  k.kind = src->kind;
+  k.t = src->t;
+  if (src->kind == RIAB_MOTION_IMPORTED) {
+    const riab_trajectory& tr = src->traj;
+    if (tr.times_dev == nullptr || tr.y_dev == nullptr || tr.M_dev == nullptr || tr.T < 4 || !(tr.t_max > 0.0))
+      return fail(RIAB_ERR_INVALID, "motion source: bad trajectory");
+    if (tr.n_traj != 1 && tr.n_traj != n_agents)
+      return fail(RIAB_ERR_INVALID, "motion source: %lld trajectories for %lld agents", (long long)tr.n_traj, n_agents);
+    k.times = tr.times_dev; k.y = tr.y_dev; k.M = tr.M_dev; k.T = tr.T; k.n_traj = tr.n_traj; k.t_max = tr.t_max;
+    return 0;
+  }
+  if (src->kind == RIAB_MOTION_FORCED) {
+    if (src->forced_dev == nullptr) return fail(RIAB_ERR_INVALID, "motion source: forced positions NULL");
+    k.forced = src->forced_dev; k.bcast = src->forced_broadcast != 0;
+    return 0;
+  }
+  return fail(RIAB_ERR_INVALID, "motion source: kind %d", src->kind);
+}
+
+// ---------------------------------------------------------------------------
+// (the motion and step arguments of MODE-0 launches, which read neither)
+const riab_motion_params kNoMotion = {};
+const riab_step_io kNoStep = {};
+
+// One population of one step, checked: its kind's constants and its output.
+struct Pop {
+  int kind = -1, n_cells = 0;
+  double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
+  OutK out;
+  PlaceConst place; GridConst grid; OvcConst ovc;
+  const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
+  const riab_ffl_cells* ffl = nullptr;
+};
+
+int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* out, const riab_neuron_noise* noise,
+             double dt, const riab_agents& ag, Pop& d) {
+  if (cells == nullptr) return fail(RIAB_ERR_INVALID, "cells NULL");
+  int rc = 0;
+  d.kind = kind;
+  if (kind == RIAB_CELLS_PLACE) {
+    const riab_place_cells* pc = (const riab_place_cells*)cells;
+    rc = make_place(pc, ek, d.place);
+    d.n_cells = pc->n_cells;
+    if (pc->description != RIAB_PC_ONE_HOT) d.bound = fmaxf(pc->min_fr, pc->max_fr);   // one_hot: post-pass spikes, dense
+  } else if (kind == RIAB_CELLS_GRID) {
+    const riab_grid_cells* gc = (const riab_grid_cells*)cells;
+    rc = make_grid(gc, ek, d.grid);
+    d.n_cells = gc->n_cells;
+    d.bound = fmaxf(gc->min_fr, gc->max_fr);
+  } else if (kind == RIAB_CELLS_OVC) {
+    rc = make_ovc((const riab_ovc_cells*)cells, ek, ag.head_direction, d.ovc);
+    d.n_cells = d.ovc.n_cells;
+  } else if (kind == RIAB_CELLS_BVC) {
+    d.bvc = (const riab_bvc_cells*)cells;
+    d.n_cells = d.bvc->n_cells;
+  } else if (kind == RIAB_CELLS_FFL) {
+    d.ffl = (const riab_ffl_cells*)cells;
+    d.n_cells = d.ffl->n_cells;
+  } else {
+    return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
+  }
+  if (rc || (rc = make_out(out, noise, d.n_cells, dt, ag.id_offset, d.out, d.bound))) return rc;
+  if (kind == RIAB_CELLS_BVC) return check_bvc(ek, d.bvc, d.bvc_scratch = out->bvc_scratch, ag.n_agents);
+  return kind == RIAB_CELLS_FFL ? check_ffl(d.ffl, d.out, ag.n_agents) : 0;
+}
+
+// One population's kernels for one step.  MODE 0: rates at the agents' positions; 1: the motion step fused in; 2: skewed
+// (rates at the current positions while the motion of the next step runs, riab_run).  BVC and FFL populations run MODE 0.
+template <int MODE>
+int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const Pop& d,
+               cudaStream_t s, BvcPipe* pipe = nullptr) {
+  const double* pos_in = (MODE == 1) ? nullptr : ag.pos;
+  if (d.kind == RIAB_CELLS_PLACE) return launch_place<MODE>(ek, ag, mp, io, d.place, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_GRID) return launch_tile<GridPolicy, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
+  if constexpr (MODE == 0) {
+    if (d.kind == RIAB_CELLS_BVC)
+      return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
+    return launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
+  } else {
+    return fail(RIAB_ERR_INVALID, "cells kind %d is launched unfused", d.kind);
+  }
+}
+
+// The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), one_hot (an
+// arg-min across cells), BVC (the latency-bound ray kernel wants all its CTAs in ONE wave: the 128-register motion code
+// would halve its occupancy) and FeedForwardLayers (they read other populations' rows, not the positions).
+bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
+  return io.collision_mask || io.first_hit || io.n_iters || d.kind == RIAB_CELLS_BVC || d.kind == RIAB_CELLS_FFL ||
+         (d.kind == RIAB_CELLS_PLACE && d.place.desc == RIAB_PC_ONE_HOT);
+}
+
+// One motion step, then population d's rates at the new positions; everything is checked before.
+int step_fused(const riab_agents* agents, const riab_env* env, const EnvK& ek, const riab_motion_params* prm,
+               const riab_step_io* io, const Pop& d, cudaStream_t s, BvcPipe* pipe = nullptr) {
+  if (!needs_motion_kernel(*io, d)) return launch_pop<1>(ek, *agents, *prm, *io, d, s);
+  const int rc = riab_agent_update(agents, env, prm, io, s);
+  return rc ? rc : launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s, pipe);
+}
+
+// riab_step_fused (fused: the motion step, then the rates) and riab_neurons_update (the rates at agents->pos)
+int neurons_update_impl(bool fused, const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
+                        const riab_step_io* io, int32_t cells_kind, const void* cells, const riab_neuron_noise* noise,
+                        const riab_rates_out* out, void* stream) {
+  EnvK ek;
+  Pop d;
+  int rc;
+  if ((rc = check_agents(agents)) || (rc = make_env(env, ek)) || (fused && (rc = check_motion(prm)))) return rc;
+  if (fused && io == nullptr) return fail(RIAB_ERR_INVALID, "io NULL");
+  if ((rc = make_pop(ek, cells_kind, cells, out, noise, fused ? prm->dt : (noise ? noise->dt : 1.0), *agents, d))) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  return fused ? step_fused(agents, env, ek, prm, io, d, s) : launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s);
+}
+
+// get_state: the rates at n_pos given positions (and head directions, egocentric cells), without noise or spikes
+int rates_at(int kind, const void* cells, const double* pos_dev, int64_t n_pos, const riab_env* env, const double* head_dir,
+             float* scratch, int32_t* first_wall, float* out_dev, int64_t ld_out, void* stream) {
+  if (n_pos == 0) return 0;
+  EnvK ek;
+  Pop d;
+  int rc;
+  if ((rc = make_env(env, ek))) return rc;
+  if (n_pos > 0 && pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "pos_dev NULL");
+  riab_rates_out ro = {};
+  ro.rates_row = out_dev; ro.ld = ld_out; ro.bvc_scratch = scratch;
+  riab_agents at = {};
+  at.n_agents = n_pos; at.pos = (double*)pos_dev; at.head_direction = (double*)head_dir;
+  if ((rc = make_pop(ek, kind, cells, &ro, nullptr, 1.0, at, d))) return rc;
+  d.first_wall = first_wall;
+  return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
+}
+
+// Row (next + k) mod rows of a ring of rows of row_len elements (next + k >= 0)
+template <class T>
+T* ring_row(T* ring, long long next_k, int rows, long long row_len) { return ring + (size_t)(next_k % rows) * row_len; }
+
+// riab_run's use of the BVC pipeline (BvcPipe).  begin() pipelines the run when every population is an allocentric BVC
+// one with a ring of >= 2 rows and the run has >= 2 steps: next to Place / Grid rate kernels (HBM- and dispatch-bound) the
+// overlapped integral just competes for the same SMs (measured slower on configs[4]).  Leaving the run joins the side
+// stream and frees the second ray buffers.
+struct PipeScope {
+  BvcPipe* pipe = nullptr;
+  cudaStream_t s = nullptr;
+  int begin(const riab_population* pops, int n_pops, long long n_agents, long long n_steps, cudaStream_t stream) {
+    if (n_pops < 1 || n_pops > PIPE_POPS || n_steps < 2) return 0;
+    for (int q = 0; q < n_pops; ++q)
+      if (pops[q].kind != RIAB_CELLS_BVC || pops[q].cells == nullptr || ((const riab_bvc_cells*)pops[q].cells)->egocentric ||
+          pops[q].ring_rows < 2 || pops[q].out.bvc_scratch == nullptr)
+        return 0;
+    static thread_local BvcPipe pipes[16];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 16) return 0;
+    BvcPipe* p = &pipes[dev];
+    if (p->side == nullptr) {
+      // keep the stream-ordered pool's memory across runs (by default it goes back to the driver at every synchronisation
+      // and each run would pay a ~1 ms cudaMalloc for its second ray buffer again)
+      cudaMemPool_t pool;
+      if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+        unsigned long long keep = ~0ull;
+        cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+      }
+      RIAB_CUDA_OK(cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking));
+      RIAB_CUDA_OK(cudaEventCreateWithFlags(&p->rays_done, cudaEventDisableTiming));
+      for (int b = 0; b < 2; ++b)
+        for (int q = 0; q < PIPE_POPS; ++q) RIAB_CUDA_OK(cudaEventCreateWithFlags(&p->int_done[b][q], cudaEventDisableTiming));
+    }
+    memset(p->used, 0, sizeof(p->used));
+    memset(p->scratch2, 0, sizeof(p->scratch2));
+    pipe = p;
+    s = stream;
+    for (int q = 0; q < n_pops; ++q) {
+      const int pid = pops[q].noise.population_id, T = ((const riab_bvc_cells*)pops[q].cells)->n_test_angles;
+      if (pid >= 0 && pid < PIPE_POPS)
+        RIAB_CUDA_OK(cudaMallocAsync((void**)&p->scratch2[pid], (size_t)riab_bvc_scratch_floats(n_agents, T) * sizeof(float), s));
+    }
+    return 0;
+  }
+  ~PipeScope() {
+    if (pipe == nullptr) return;
+    for (int b = 0; b < 2; ++b)
+      for (int q = 0; q < PIPE_POPS; ++q)
+        if (pipe->used[b][q]) cudaStreamWaitEvent(s, pipe->int_done[b][q], 0);
+    for (int q = 0; q < PIPE_POPS; ++q)
+      if (pipe->scratch2[q] != nullptr) { cudaFreeAsync(pipe->scratch2[q], s); pipe->scratch2[q] = nullptr; }
+  }
+};
+
+// Whether riab_run takes the whole run as ONE launch (k_step MODE 3, or 4 with a motion source; see RunK) under the
+// conditions DESIGN.md §4 lists; a motion source's whole run does not look at xi or the parity taps.  d: population 0 on
+// its ring bases (make_out's alignment checks then hold for every row).
+int whole_run_applies(const EnvK& ek, const riab_agents& ag, const riab_motion_params& prm, const riab_step_io& io,
+                      const riab_motion_source* src, const riab_population* pops, int n_pops,
+                      const riab_agent_history* hist, Pop& d, bool& yes) {
+  yes = false;
+  if (n_pops != 1 || getenv("RIAB_NO_WHOLE_RUN") != nullptr || io.drift_velocity != nullptr || io.pos_mirror != nullptr ||
+      (src == nullptr && (io.xi != nullptr || io.collision_mask || io.first_hit || io.n_iters)))
+    return 0;
+  const riab_population& pp = pops[0];
+  if ((pp.kind != RIAB_CELLS_PLACE && pp.kind != RIAB_CELLS_GRID) || pp.rates_ring == nullptr || pp.ring_rows <= 0 ||
+      pp.noise.noise_std != 0.f)
+    return 0;
+  riab_rates_out ro = pp.out;
+  ro.rates_row = pp.rates_ring; ro.spikes_row = pp.spikes_ring;
+  riab_neuron_noise nz = pp.noise;
+  nz.dt = prm.dt;
+  int rc;
+  if ((rc = make_pop(ek, pp.kind, pp.cells, &ro, &nz, prm.dt, ag, d))) return rc;
+  const OutK& ok = d.out;
+  const long long A = ag.n_agents;
+  const bool place = pp.kind == RIAB_CELLS_PLACE;
+  const int ct = (place ? d.place.n_pad : d.grid.n_pad) / 4;
+  const bool rows_ok = ((A * ok.ld) % 4 == 0) && ((A * ok.spike_ld) % 4 == 0);        // every ring row stays 16-byte aligned
+  const bool lean = ok.vec_ok && rows_ok && (d.n_cells % 4 == 0) && ct <= RW * 32 &&
+                    (ok.spikes == nullptr || (ag.id_offset & 1) == 0) &&
+                    (4 % lean_groups(ct, 8) == 0) && (4 % lean_groups(ct, 4) == 0);      // groups divide the 4 producers
+  // with a spike ring of one row a producer's clear of step s+1's rows could land before the consumers' RED.OR of step s
+  yes = !(place && d.place.desc == RIAB_PC_ONE_HOT) && lean && (hist == nullptr || hist->ring == nullptr || hist->ring_rows > 0) &&
+        (pp.spikes_ring == nullptr || pp.ring_rows >= 2);
+  return 0;
+}
+
+// The schedule of a riab_run: WHOLE (one launch), SKEWED or PLAIN, and the order of a step's populations.
+struct RunPlan {
+  enum { PLAIN, SKEWED, WHOLE } sched = PLAIN;
+  bool motion_alone = false;      // PLAIN: the motion kernel runs on its own first, else population 0's launch takes the step
+  std::vector<int> order;
+  Pop whole;                      // WHOLE: the population
+};
+
+int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& prm, const riab_step_io& io,
+             const riab_motion_source* src, const riab_population* pops, int n_pops, const riab_agent_history* hist,
+             RunPlan& plan) {
+  bool whole;
+  int rc;
+  if ((rc = whole_run_applies(ek, ag, prm, io, src, pops, n_pops, hist, plan.whole, whole))) return rc;
+  if (whole) {
+    plan.sched = RunPlan::WHOLE;
+    return 0;
+  }
+  // A FeedForwardLayer reads other populations' rows of the same step and masks the agents whose position of that step is
+  // NaN, so an Agent with one keeps the plain schedule: the positions advance before any population of the step.
+  bool any_ffl = false;
+  for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
+  const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
+                       ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
+  // Skewed schedule (population 0 is a Place / Grid / OVC population): motion(0) alone, then per step one kernel that
+  // evaluates rates(s) of the current positions while its producer warps already run motion(s+1); the last step is rates
+  // only.  Same results as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source
+  // keeps the plain schedule (its motion kernel is cheap next to the rates).
+  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && !any_ffl && io.xi == nullptr &&
+                    !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr;
+  plan.sched = skew ? RunPlan::SKEWED : RunPlan::PLAIN;
+  plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || pops[0].kind == RIAB_CELLS_FFL);
+  // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
+  // FeedForwardLayers in registration order, after every row they read of this step exists
+  for (int p = skew ? 1 : 0; p < n_pops; ++p)
+    if (pops[p].kind != RIAB_CELLS_FFL) plan.order.push_back(p);
+  if (skew) plan.order.push_back(0);
+  for (int p = 0; p < n_pops; ++p)
+    if (pops[p].kind == RIAB_CELLS_FFL) plan.order.push_back(p);
+  return 0;
+}
+
+// riab_run / riab_run_src.  src: NULL for the random motion, else an imported trajectory (already checked).
+int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
+             const riab_motion_source* src, const riab_population* pops, int32_t n_pops,
+             const riab_agent_history* hist, int64_t n_steps, void* stream) {
+  if (agents == nullptr || io == nullptr || n_pops < 0 || (n_pops > 0 && pops == nullptr))
+    return fail(RIAB_ERR_INVALID, "riab_run: bad argument");
+  if (n_steps <= 0) return 0;
+  EnvK ek;
+  RunPlan plan;
+  int rc;
+  if ((rc = check_agents(agents)) || (rc = make_env(env, ek)) || (rc = check_motion(prm)) ||
+      (rc = plan_run(ek, *agents, *prm, *io, src, pops, n_pops, hist, plan)))
+    return rc;
+  const int64_t A = agents->n_agents;
+  const bool agent_ring = hist != nullptr && hist->ring != nullptr && hist->ring_rows > 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (plan.sched == RunPlan::WHOLE) {
+    const riab_population& pp = pops[0];
+    const Pop& d = plan.whole;
+    RunK run;
+    memset(&run, 0, sizeof(run));
+    run.n_steps = n_steps;
+    run.rates_ring = pp.rates_ring; run.spikes_ring = pp.spikes_ring;
+    run.ring_rows = pp.ring_rows; run.ring_next = pp.ring_next;
+    if (agent_ring) {
+      run.hist_ring = hist->ring; run.hist_rows = hist->ring_rows; run.hist_next = hist->ring_next;
+    }
+    riab_step_io io0 = *io;
+    io0.history_row = nullptr;
+    if (src != nullptr && (rc = make_src(src, A, run.src))) return rc;
+    if (pp.kind == RIAB_CELLS_PLACE)
+      return src ? launch_place<4>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run)
+                 : launch_place<3>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run);
+    return src ? launch_tile<GridPolicy, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
+               : launch_tile<GridPolicy, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
+  }
+
+  riab_motion_source src_st;                          // step st's clock: t_st = t_{st-1} + dt
+  if (src != nullptr) src_st = *src;
+  auto step_io = [&](int64_t st) {
+    riab_step_io sio = *io;
+    sio.step = io->step + (uint64_t)st;
+    sio.history_row = agent_ring ? ring_row(hist->ring, hist->ring_next + st, hist->ring_rows, A * 8) : nullptr;
+    return sio;
+  };
+  if (plan.sched == RunPlan::SKEWED) {
+    const riab_step_io s0 = step_io(0);
+    if ((rc = riab_agent_update(agents, env, prm, &s0, stream))) return rc;
+  }
+  PipeScope pipe;
+  if ((rc = pipe.begin(pops, n_pops, A, n_steps, s))) return rc;
+  for (int64_t st = 0; st < n_steps; ++st) {
+    if (pipe.pipe) pipe.pipe->step = st;
+    const riab_step_io sio = step_io(st);
+    if (plan.motion_alone) {
+      if (src == nullptr) {
+        rc = riab_agent_update(agents, env, prm, &sio, stream);
+      } else {
+        rc = riab_agent_update_src(agents, env, prm, &sio, &src_st, stream);
+        src_st.t = src_st.t + prm->dt;
+      }
+      if (rc) return rc;
+    }
+    for (const int p : plan.order) {
+      const riab_population& pp = pops[p];
+      if (pp.rates_ring == nullptr || pp.ring_rows <= 0) return fail(RIAB_ERR_INVALID, "population %d: no rates ring", p);
+      riab_rates_out ro = pp.out;                   // on the ring bases: make_out's alignment checks hold for every row
+      ro.rates_row = pp.rates_ring; ro.spikes_row = pp.spikes_ring;
+      riab_neuron_noise nz = pp.noise;
+      nz.step = pp.noise.step + (uint64_t)st; nz.dt = prm->dt;
+      riab_ffl_cells fc;
+      if (pp.kind == RIAB_CELLS_FFL) {
+        // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
+        // previous step's: before the first step, the row the caller passed
+        fc = *(const riab_ffl_cells*)pp.cells;
+        for (int i = 0; i < fc.n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
+          riab_ffl_input& in = fc.inputs[i];
+          if (in.population < 0 || in.population >= n_pops || (in.lag == 0) != (in.population < p) || in.lag < 0 || in.lag > 1)
+            return fail(RIAB_ERR_INVALID, "population %d: FeedForwardLayer input %d (population %d, lag %d) out of order", p, i,
+                        in.population, in.lag);
+          const riab_population& ip = pops[in.population];
+          if (in.lag == 1 && st == 0) continue;
+          if (in.lag == 1 && ip.ring_rows < 2)
+            return fail(RIAB_ERR_INVALID, "population %d feeds a FeedForwardLayer with one step of lag: it needs 2 ring rows", in.population);
+          in.rows_dev = ring_row(ip.rates_ring, ip.ring_next + st - in.lag, ip.ring_rows, A * ip.out.ld);
+          in.ld = ip.out.ld;
+        }
+      }
+      Pop d;
+      if ((rc = make_pop(ek, pp.kind, pp.kind == RIAB_CELLS_FFL ? (const void*)&fc : pp.cells, &ro, &nz, prm->dt, *agents, d)))
+        return rc;
+      d.out.rates = ring_row(pp.rates_ring, pp.ring_next + st, pp.ring_rows, A * pp.out.ld);
+      if (d.out.spikes != nullptr) d.out.spikes = ring_row(pp.spikes_ring, pp.ring_next + st, pp.ring_rows, A * d.out.spike_ld);
+      if (p != 0 || plan.motion_alone) rc = launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s, pipe.pipe);
+      else if (plan.sched == RunPlan::PLAIN) rc = step_fused(agents, env, ek, prm, &sio, d, s, pipe.pipe);
+      else if (st + 1 < n_steps) rc = launch_pop<2>(ek, *agents, *prm, step_io(st + 1), d, s);   // its motion: step st+1's
+      else rc = launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s);
+      if (rc) return rc;
+    }
+  }
+  return 0;
+}
+
+// ---- host-buffer motion step on two streams (see include/riab_b200.h)
+struct HostIo {
+  cudaStream_t side = nullptr;
+  cudaEvent_t up_done = nullptr, motion_done = nullptr, pos_done = nullptr;
+  bool pos_inflight = false;
+};
+thread_local HostIo g_hostio[16];
+int hostio(HostIo*& h) {
+  int dev = 0;
+  RIAB_CUDA_OK(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 16) return fail(RIAB_ERR_UNSUPPORTED, "device ordinal %d", dev);
+  h = &g_hostio[dev];
+  if (h->side == nullptr) {
+    RIAB_CUDA_OK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
+    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->up_done, cudaEventDisableTiming));
+    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->motion_done, cudaEventDisableTiming));
+    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->pos_done, cudaEventDisableTiming));
+  }
+  return 0;
+}
 }  // namespace
 
 // ===========================================================================
 extern "C" {
+
 
 int riab_abi_version(void) { return RIAB_ABI_VERSION; }
 const char* riab_last_error(void) { return g_err; }
@@ -1995,28 +2385,6 @@ int riab_trajectory_build(const riab_trajectory* tr, const double* times_host, v
   return 0;
 }
 
-}  // extern "C"
-static int make_src(const riab_motion_source* src, long long n_agents, SrcK& k) {
-  memset(&k, 0, sizeof(k));
-  k.kind = src->kind;
-  k.t = src->t;
-  if (src->kind == RIAB_MOTION_IMPORTED) {
-    const riab_trajectory& tr = src->traj;
-    if (tr.times_dev == nullptr || tr.y_dev == nullptr || tr.M_dev == nullptr || tr.T < 4 || !(tr.t_max > 0.0))
-      return fail(RIAB_ERR_INVALID, "motion source: bad trajectory");
-    if (tr.n_traj != 1 && tr.n_traj != n_agents)
-      return fail(RIAB_ERR_INVALID, "motion source: %lld trajectories for %lld agents", (long long)tr.n_traj, n_agents);
-    k.times = tr.times_dev; k.y = tr.y_dev; k.M = tr.M_dev; k.T = tr.T; k.n_traj = tr.n_traj; k.t_max = tr.t_max;
-    return 0;
-  }
-  if (src->kind == RIAB_MOTION_FORCED) {
-    if (src->forced_dev == nullptr) return fail(RIAB_ERR_INVALID, "motion source: forced positions NULL");
-    k.forced = src->forced_dev; k.bcast = src->forced_broadcast != 0;
-    return 0;
-  }
-  return fail(RIAB_ERR_INVALID, "motion source: kind %d", src->kind);
-}
-extern "C" {
 
 int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
                           const riab_step_io* io, const riab_motion_source* src, void* stream) {
@@ -2130,21 +2498,7 @@ int riab_place_pack(const double* centres, const double* widths, int32_t n, cons
 
 int riab_place_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_place_cells* pc,
                      float* out_dev, int64_t ld_out, void* stream) {
-  if (n_pos == 0) return 0;
-  EnvK ek;
-  PlaceConst c;
-  OutK ok;
-  int rc;
-  if ((rc = make_env(env, ek)) || (rc = make_place(pc, ek, c))) return rc;
-  if (n_pos > 0 && pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "pos_dev NULL");
-  riab_rates_out ro;
-  memset(&ro, 0, sizeof(ro));
-  ro.rates_row = out_dev; ro.ld = ld_out;
-  if ((rc = make_out(&ro, nullptr, pc->n_cells, 1.0, 0, ok))) return rc;
-  riab_agents ag; memset(&ag, 0, sizeof(ag));
-  riab_motion_params mp; memset(&mp, 0, sizeof(mp));
-  riab_step_io io; memset(&io, 0, sizeof(io));
-  return launch_place<0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
+  return rates_at(RIAB_CELLS_PLACE, pc, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ------------------------------------------------------------------ GridCells
@@ -2177,21 +2531,7 @@ int riab_grid_pack(const double* gridscales, const double* phase_offsets, const 
 
 int riab_grid_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_grid_cells* gc,
                     float* out_dev, int64_t ld_out, void* stream) {
-  if (n_pos == 0) return 0;
-  EnvK ek;
-  GridConst c;
-  OutK ok;
-  int rc;
-  if ((rc = make_env(env, ek)) || (rc = make_grid(gc, ek, c))) return rc;
-  if (n_pos > 0 && pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "pos_dev NULL");
-  riab_rates_out ro;
-  memset(&ro, 0, sizeof(ro));
-  ro.rates_row = out_dev; ro.ld = ld_out;
-  if ((rc = make_out(&ro, nullptr, gc->n_cells, 1.0, 0, ok))) return rc;
-  riab_agents ag; memset(&ag, 0, sizeof(ag));
-  riab_motion_params mp; memset(&mp, 0, sizeof(mp));
-  riab_step_io io; memset(&io, 0, sizeof(io));
-  return launch_tile<GridPolicy, 0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
+  return rates_at(RIAB_CELLS_GRID, gc, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ------------------------------------------------------------------------ BVC
@@ -2281,22 +2621,8 @@ int riab_bvc_pack(const double* mu_d, const double* mu_t, const double* sg_d, co
 int riab_bvc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_bvc_cells* bvc,
                    float* scratch_dev, int32_t* first_wall_dev, const double* head_direction_dev, float* out_dev,
                    int64_t ld_out, void* stream) {
-  if (n_pos == 0) return 0;
-  EnvK ek;
-  OutK ok;
-  int rc;
-  if ((rc = make_env(env, ek))) return rc;
-  if (bvc == nullptr) return fail(RIAB_ERR_INVALID, "bvc NULL");
-  if (n_pos > 0 && pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "pos_dev NULL");
-  riab_rates_out ro;
-  memset(&ro, 0, sizeof(ro));
-  ro.rates_row = out_dev; ro.ld = ld_out;
-  if ((rc = make_out(&ro, nullptr, bvc->n_cells, 1.0, 0, ok))) return rc;
-  riab_agents ag; memset(&ag, 0, sizeof(ag));
-  riab_motion_params mp; memset(&mp, 0, sizeof(mp));
-  riab_step_io io; memset(&io, 0, sizeof(io));
-  return launch_bvc<false>(ek, ag, mp, io, bvc, ok, pos_dev, n_pos, scratch_dev, first_wall_dev, head_direction_dev,
-                           (cudaStream_t)stream);
+  return rates_at(RIAB_CELLS_BVC, bvc, pos_dev, n_pos, env, head_direction_dev, scratch_dev, first_wall_dev, out_dev, ld_out,
+                  stream);
 }
 
 // ------------------------------------------------------------ ObjectVectorCells
@@ -2324,21 +2650,7 @@ int riab_ovc_pack(const double* tuning_distances, const double* tuning_angles, c
 
 int riab_ovc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_ovc_cells* ovc,
                    const double* head_direction_dev, float* out_dev, int64_t ld_out, void* stream) {
-  if (n_pos == 0) return 0;
-  EnvK ek;
-  OvcConst c;
-  OutK ok;
-  int rc;
-  if ((rc = make_env(env, ek)) || (rc = make_ovc(ovc, ek, head_direction_dev, c))) return rc;
-  if (n_pos > 0 && pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "pos_dev NULL");
-  riab_rates_out ro;
-  memset(&ro, 0, sizeof(ro));
-  ro.rates_row = out_dev; ro.ld = ld_out;
-  if ((rc = make_out(&ro, nullptr, ovc->n_cells, 1.0, 0, ok))) return rc;
-  riab_agents ag; memset(&ag, 0, sizeof(ag));
-  riab_motion_params mp; memset(&mp, 0, sizeof(mp));
-  riab_step_io io; memset(&io, 0, sizeof(io));
-  return launch_tile<OvcPolicy, 0>(ek, ag, mp, io, c, ok, pos_dev, n_pos, (cudaStream_t)stream);
+  return rates_at(RIAB_CELLS_OVC, ovc, pos_dev, n_pos, env, head_direction_dev, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ------------------------------------------------------------ FeedForwardLayer
@@ -2381,314 +2693,25 @@ int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_
   if (ffl == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_ffl_rates: bad argument");
   OutK ok;
   int rc;
-  if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok))) return rc;
+  if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
+      (rc = check_ffl(ffl, ok, n_rows))) return rc;
   return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
 }
 
 // ----------------------------------------------------------------- fused step
-// MODE 1: motion + rates of one population; 0: rates for agents->pos as it is; 2: skewed (riab_run).
-}  // extern "C"
-template <int MODE>
-static int neurons_update_impl(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
-                               const riab_step_io* io, int32_t cells_kind, const void* cells,
-                               const riab_neuron_noise* noise, const riab_rates_out* out, void* stream) {
-  EnvK ek;
-  OutK ok;
-  int rc;
-  if ((rc = check_agents(agents)) || (rc = make_env(env, ek))) return rc;
-  if (MODE != 0 && (rc = check_motion(prm))) return rc;
-  if (cells == nullptr || (MODE != 0 && io == nullptr)) return fail(RIAB_ERR_INVALID, "io / cells NULL");
-  if (MODE == 1 && (io->collision_mask || io->first_hit || io->n_iters) && cells_kind != RIAB_CELLS_BVC) {
-    // parity taps are only implemented in the stand-alone motion kernel
-    if ((rc = riab_agent_update(agents, env, prm, io, stream))) return rc;
-    return neurons_update_impl<0>(agents, env, prm, io, cells_kind, cells, noise, out, stream);
-  }
-  riab_motion_params mp0; memset(&mp0, 0, sizeof(mp0));
-  riab_step_io io0; memset(&io0, 0, sizeof(io0));
-  const riab_motion_params& mp = (MODE != 0) ? *prm : mp0;
-  const riab_step_io& sio = (MODE != 0) ? *io : io0;
-  const double dt = (prm != nullptr) ? prm->dt : (noise ? noise->dt : 1.0);
-  const double* pos_in = (MODE == 1) ? nullptr : agents->pos;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (cells_kind == RIAB_CELLS_PLACE) {
-    const riab_place_cells* pc = (const riab_place_cells*)cells;
-    PlaceConst c;
-    const bool onehot = pc != nullptr && pc->description == RIAB_PC_ONE_HOT;     // post-pass spikes (k_finish_rows): dense
-    if ((rc = make_place(pc, ek, c)) ||
-        (rc = make_out(out, noise, pc->n_cells, dt, agents->id_offset, ok, onehot ? -1.0 : (double)fmaxf(pc->min_fr, pc->max_fr)))) return rc;
-    if (c.desc == RIAB_PC_ONE_HOT) {             // arg-min across cells: its own kernel after the motion kernel
-      if (MODE == 2) return fail(RIAB_ERR_UNSUPPORTED, "one_hot populations are stepped unskewed");
-      if (MODE == 1 && (rc = riab_agent_update(agents, env, prm, io, stream))) return rc;
-      return launch_place<0>(ek, *agents, mp0, io0, c, ok, agents->pos, agents->n_agents, s);
-    }
-    return launch_place<MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
-  }
-  if (cells_kind == RIAB_CELLS_GRID) {
-    const riab_grid_cells* gc = (const riab_grid_cells*)cells;
-    GridConst c;
-    if ((rc = make_grid(gc, ek, c)) ||
-        (rc = make_out(out, noise, gc->n_cells, dt, agents->id_offset, ok, (double)fmaxf(gc->min_fr, gc->max_fr)))) return rc;
-    return launch_tile<GridPolicy, MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
-  }
-  if (cells_kind == RIAB_CELLS_BVC) {
-    if (MODE == 2) return fail(RIAB_ERR_UNSUPPORTED, "BVC populations are stepped unskewed");
-    const riab_bvc_cells* bvc = (const riab_bvc_cells*)cells;
-    if ((rc = make_out(out, noise, bvc->n_cells, dt, agents->id_offset, ok))) return rc;
-    // The ray kernel wants all its CTAs resident in ONE wave (the float64 ray chains are latency-bound);
-    // fusing the 128-register motion code into it halves its occupancy and adds a tail wave, so the
-    // motion runs as its own kernel first.
-    if (MODE == 1 && (rc = riab_agent_update(agents, env, prm, io, stream))) return rc;
-    return launch_bvc<false>(ek, *agents, mp0, io0, bvc, ok, agents->pos, agents->n_agents, out->bvc_scratch, nullptr,
-                             agents->head_direction, s);
-  }
-  if (cells_kind == RIAB_CELLS_OVC) {
-    const riab_ovc_cells* oc = (const riab_ovc_cells*)cells;
-    OvcConst c;
-    if ((rc = make_ovc(oc, ek, agents->head_direction, c)) || (rc = make_out(out, noise, oc->n_cells, dt, agents->id_offset, ok))) return rc;
-    return launch_tile<OvcPolicy, MODE>(ek, *agents, mp, sio, c, ok, pos_in, agents->n_agents, s);
-  }
-  if (cells_kind == RIAB_CELLS_FFL) {
-    if (MODE == 2) return fail(RIAB_ERR_UNSUPPORTED, "FeedForwardLayer populations are stepped unskewed");
-    const riab_ffl_cells* fc = (const riab_ffl_cells*)cells;
-    if ((rc = make_out(out, noise, fc->n_cells, dt, agents->id_offset, ok))) return rc;
-    // the layer reads other populations' rows, not the positions (except for its NaN mask): the motion runs first
-    if (MODE == 1 && (rc = riab_agent_update(agents, env, prm, io, stream))) return rc;
-    return launch_ffl(fc, agents->n_agents, agents->pos, ok, s);
-  }
-  return fail(RIAB_ERR_INVALID, "bad cells_kind %d", cells_kind);
-}
-extern "C" {
 
 int riab_step_fused(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
                     const riab_step_io* io, int32_t cells_kind, const void* cells, const riab_neuron_noise* noise,
                     const riab_rates_out* out, void* stream) {
-  return neurons_update_impl<1>(agents, env, prm, io, cells_kind, cells, noise, out, stream);
+  return neurons_update_impl(true, agents, env, prm, io, cells_kind, cells, noise, out, stream);
 }
 
 int riab_neurons_update(const riab_agents* agents, const riab_env* env, int32_t cells_kind, const void* cells,
                         const riab_neuron_noise* noise, const riab_rates_out* out, void* stream) {
-  return neurons_update_impl<0>(agents, env, nullptr, nullptr, cells_kind, cells, noise, out, stream);
+  return neurons_update_impl(false, agents, env, nullptr, nullptr, cells_kind, cells, noise, out, stream);
 }
 
-}  // extern "C"
-// riab_run / riab_run_src.  src: NULL for the random motion, else an imported trajectory (already checked).
-static int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
-                    const riab_motion_source* src, const riab_population* pops, int32_t n_pops,
-                    const riab_agent_history* hist, int64_t n_steps, void* stream) {
-  if (agents == nullptr || io == nullptr || n_pops < 0 || (n_pops > 0 && pops == nullptr))
-    return fail(RIAB_ERR_INVALID, "riab_run: bad argument");
-  const int64_t A = agents->n_agents;
-  // Skewed schedule (population 0 is a Place/Grid population): motion(0) alone, then per step one
-  // kernel that evaluates rates(s) of the current positions while its producer warps already run
-  // motion(s+1); the last step is rates only.  Same results as the plain sequence, but the
-  // float64 motion chain never gates the rate warps.
-  const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
-                       ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
-  // A FeedForwardLayer reads other populations' rows of the same step and masks the agents whose position of that step is
-  // NaN, so an Agent with one keeps the plain schedule: the positions advance before any population of the step.
-  bool any_ffl = false;
-  for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
-  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && !any_ffl && n_steps >= 1 &&
-                    io->xi == nullptr && !io->collision_mask && !io->first_hit && !io->n_iters && src == nullptr;
-  // a motion source keeps the plain schedule (its motion kernel is cheap next to the rates): per step, the motion kernel
-  // of the step and then every population, except for the whole-run case below.  Step st's clock: t_st = t_{st-1} + dt
-  riab_motion_source src_st;
-  if (src != nullptr) src_st = *src;
-  auto motion = [&](const riab_step_io& sio) {
-    if (src == nullptr) return riab_agent_update(agents, env, prm, &sio, stream);
-    const int r = riab_agent_update_src(agents, env, prm, &sio, &src_st, stream);
-    src_st.t = src_st.t + prm->dt;
-    return r;
-  };
-  const bool whole = src == nullptr ? skew : (n_pops >= 1 && n_steps >= 1 && !any_ffl);
-  auto step_io = [&](int64_t st) {
-    riab_step_io sio = *io;
-    sio.step = io->step + (uint64_t)st;
-    sio.history_row = nullptr;
-    if (hist != nullptr && hist->ring != nullptr && hist->ring_rows > 0)
-      sio.history_row = hist->ring + (size_t)((hist->ring_next + st) % hist->ring_rows) * A * 8;
-    return sio;
-  };
-  int rc;
-  // ---- a single Place / Grid population: the whole run as ONE launch (k_step MODE 3, see RunK) where the lean consumer
-  // loop applies: vector-aligned rows, whole 4-cell groups, all cells in one register set, consumer groups that divide the
-  // producers, no OU noise, no parity taps, and no spike ring of a single row.  Rings of any depth may wrap: a tile's rows
-  // of step s are written by one consumer group in step order.  But a producer clears its tile's spike rows of step s+1 as
-  // soon as its private ring (at most 2 records) has room, while the consumers may still RED.OR step s's thinned spikes;
-  // with ring_rows >= 2 those are different rows, with one row nothing orders the clear after the ORs, so that case takes
-  // the per-step loop (stream-ordered launches)
-  if (n_pops == 1 && whole && getenv("RIAB_NO_WHOLE_RUN") == nullptr && io->drift_velocity == nullptr && io->pos_mirror == nullptr) {
-    const riab_population& pp = pops[0];
-    EnvK ek;
-    OutK ok;
-    if ((rc = check_agents(agents)) || (rc = make_env(env, ek)) || (rc = check_motion(prm))) return rc;
-    const bool place = pp.kind == RIAB_CELLS_PLACE, grid = pp.kind == RIAB_CELLS_GRID;
-    if ((place || grid) && pp.rates_ring != nullptr && pp.ring_rows > 0 && pp.noise.noise_std == 0.f) {
-      PlaceConst pcst;
-      GridConst gcst;
-      int n_cells = 0, n_pad = 0;
-      double bound = -1.0;
-      bool ok_cells = true;
-      if (place) {
-        const riab_place_cells* pc = (const riab_place_cells*)pp.cells;
-        if ((rc = make_place(pc, ek, pcst))) return rc;
-        n_cells = pc->n_cells; n_pad = pc->n_pad; bound = (double)fmaxf(pc->min_fr, pc->max_fr);
-        ok_cells = pc->description != RIAB_PC_ONE_HOT;
-      } else {
-        const riab_grid_cells* gc = (const riab_grid_cells*)pp.cells;
-        if ((rc = make_grid(gc, ek, gcst))) return rc;
-        n_cells = gc->n_cells; n_pad = gc->n_pad; bound = (double)fmaxf(gc->min_fr, gc->max_fr);
-      }
-      riab_rates_out ro = pp.out;
-      ro.rates_row = pp.rates_ring;                                    // (alignment / vector checks of make_out)
-      ro.spikes_row = pp.spikes_ring;
-      riab_neuron_noise nz = pp.noise;
-      nz.dt = prm->dt;
-      if ((rc = make_out(&ro, &nz, n_cells, prm->dt, agents->id_offset, ok, bound))) return rc;
-      const int ct = n_pad / 4;
-      const bool rows_ok = ((A * ok.ld) % 4 == 0) && ((A * ok.spike_ld) % 4 == 0);        // every ring row stays 16-byte aligned
-      const bool lean = ok_cells && ok.vec_ok && rows_ok && (n_cells % 4 == 0) && ct <= RW * 32 &&
-                        (ok.spikes == nullptr || (agents->id_offset & 1) == 0) &&
-                        (4 % lean_groups(ct, 8) == 0) && (4 % lean_groups(ct, 4) == 0);      // groups divide the 4 producers
-      const bool hist_ok = hist == nullptr || hist->ring == nullptr || hist->ring_rows > 0;
-      const bool spike_ring_ok = pp.spikes_ring == nullptr || pp.ring_rows >= 2;
-      if (lean && hist_ok && spike_ring_ok) {
-        RunK run;
-        memset(&run, 0, sizeof(run));
-        run.n_steps = n_steps;
-        run.rates_ring = pp.rates_ring; run.spikes_ring = pp.spikes_ring;
-        run.ring_rows = pp.ring_rows; run.ring_next = pp.ring_next;
-        if (hist != nullptr && hist->ring != nullptr && hist->ring_rows > 0) {
-          run.hist_ring = hist->ring; run.hist_rows = hist->ring_rows; run.hist_next = hist->ring_next;
-        }
-        riab_step_io io0 = *io;
-        io0.history_row = nullptr;
-        cudaStream_t s = (cudaStream_t)stream;
-        if (src != nullptr) {
-          if ((rc = make_src(src, A, run.src))) return rc;
-          if (place) return launch_place<4>(ek, *agents, *prm, io0, pcst, ok, nullptr, A, s, &run);
-          return launch_tile<GridPolicy, 4>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
-        }
-        if (place) return launch_place<3>(ek, *agents, *prm, io0, pcst, ok, nullptr, A, s, &run);
-        return launch_tile<GridPolicy, 3>(ek, *agents, *prm, io0, gcst, ok, nullptr, A, s, &run);
-      }
-    }
-  }
-  if (skew) {
-    const riab_step_io s0 = step_io(0);
-    if ((rc = riab_agent_update(agents, env, prm, &s0, stream))) return rc;
-  }
-  // ---- BoundaryVectorCells: pipeline rays(s+1) against the integral of step s (see BvcPipe)
-  static thread_local BvcPipe pipes[16];
-  BvcPipe* pipe = nullptr;
-  {
-    int dev = 0;
-    // only when every population is a BoundaryVectorCells one: next to Place / Grid rate kernels (HBM- and dispatch-bound) the
-    // overlapped integral just competes for the same SMs (measured slower on configs[4])
-    bool want = n_pops >= 1;
-    for (int p = 0; p < n_pops; ++p)
-      want = want && p < PIPE_POPS && (pops[p].kind == RIAB_CELLS_BVC && pops[p].cells != nullptr && !((const riab_bvc_cells*)pops[p].cells)->egocentric &&
-                                       pops[p].ring_rows >= 2 && pops[p].out.bvc_scratch != nullptr);
-    if (want && n_steps >= 2 && getenv("RIAB_NO_BVC_PIPELINE") == nullptr && cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev < 16) {
-      pipe = &pipes[dev];
-      if (pipe->side == nullptr) {
-        // keep the stream-ordered pool's memory across runs (by default it goes back to the driver at every synchronisation
-        // and each run would pay a ~1 ms cudaMalloc for its second ray buffer again)
-        cudaMemPool_t pool;
-        if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-          unsigned long long keep = ~0ull;
-          cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-        }
-        RIAB_CUDA_OK(cudaStreamCreateWithFlags(&pipe->side, cudaStreamNonBlocking));
-        RIAB_CUDA_OK(cudaEventCreateWithFlags(&pipe->rays_done, cudaEventDisableTiming));
-        for (int b = 0; b < 2; ++b)
-          for (int p = 0; p < PIPE_POPS; ++p) RIAB_CUDA_OK(cudaEventCreateWithFlags(&pipe->int_done[b][p], cudaEventDisableTiming));
-      }
-      for (int b = 0; b < 2; ++b)
-        for (int p = 0; p < PIPE_POPS; ++p) pipe->used[b][p] = false;
-      for (int p = 0; p < PIPE_POPS; ++p) pipe->scratch2[p] = nullptr;
-      for (int p = 0; p < n_pops && p < PIPE_POPS; ++p) {
-        if (pops[p].kind != RIAB_CELLS_BVC || pops[p].cells == nullptr || pops[p].ring_rows < 2 || pops[p].out.bvc_scratch == nullptr) continue;
-        const riab_bvc_cells* bc = (const riab_bvc_cells*)pops[p].cells;
-        if (bc->egocentric) continue;
-        const int pid = pops[p].noise.population_id;
-        if (pid < 0 || pid >= PIPE_POPS) continue;
-        RIAB_CUDA_OK(cudaMallocAsync((void**)&pipe->scratch2[pid], (size_t)riab_bvc_scratch_floats(A, bc->n_test_angles) * sizeof(float),
-                                     (cudaStream_t)stream));
-      }
-    }
-  }
-  struct PipeGuard {                                      // leaves riab_run: join the side stream, free the second buffers
-    BvcPipe* p; cudaStream_t s;
-    ~PipeGuard() {
-      g_pipe = nullptr;
-      if (p == nullptr) return;
-      for (int b = 0; b < 2; ++b)
-        for (int q = 0; q < PIPE_POPS; ++q)
-          if (p->used[b][q]) cudaStreamWaitEvent(s, p->int_done[b][q], 0);
-      for (int q = 0; q < PIPE_POPS; ++q)
-        if (p->scratch2[q] != nullptr) { cudaFreeAsync(p->scratch2[q], s); p->scratch2[q] = nullptr; }
-    }
-  } guard{pipe, (cudaStream_t)stream};
-  g_pipe = pipe;
-  for (int64_t st = 0; st < n_steps; ++st) {
-    if (pipe) pipe->step = st;
-    const riab_step_io sio = step_io(st);
-    if (n_pops == 0 || src != nullptr) {
-      if ((rc = motion(sio))) return rc;
-      if (n_pops == 0) continue;
-    }
-    // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
-    // FeedForwardLayers in registration order, after every row they read of this step exists
-    if (!skew && src == nullptr && pops[0].kind == RIAB_CELLS_FFL && (rc = riab_agent_update(agents, env, prm, &sio, stream))) return rc;
-    for (int pi = 0; pi < 2 * n_pops; ++pi) {
-      const int p = pi >= n_pops ? pi - n_pops : (skew ? ((pi + 1) % n_pops) : pi);
-      const riab_population& pp = pops[p];
-      if ((pp.kind == RIAB_CELLS_FFL) != (pi >= n_pops)) continue;
-      if (pp.rates_ring == nullptr || pp.ring_rows <= 0) return fail(RIAB_ERR_INVALID, "population %d: no rates ring", p);
-      const size_t slot = (size_t)((pp.ring_next + st) % pp.ring_rows);
-      riab_rates_out ro = pp.out;
-      ro.rates_row = pp.rates_ring + slot * A * pp.out.ld;
-      int n_cells = 0;
-      if (pp.kind == RIAB_CELLS_PLACE) n_cells = ((const riab_place_cells*)pp.cells)->n_cells;
-      else if (pp.kind == RIAB_CELLS_GRID) n_cells = ((const riab_grid_cells*)pp.cells)->n_cells;
-      else if (pp.kind == RIAB_CELLS_BVC) n_cells = ((const riab_bvc_cells*)pp.cells)->n_cells;
-      else if (pp.kind == RIAB_CELLS_OVC) n_cells = ((const riab_ovc_cells*)pp.cells)->n_cells;
-      else if (pp.kind == RIAB_CELLS_FFL) n_cells = ((const riab_ffl_cells*)pp.cells)->n_cells;
-      ro.spikes_row = pp.spikes_ring ? pp.spikes_ring + slot * A * (size_t)(4 * ((n_cells + 127) / 128)) : nullptr;
-      riab_neuron_noise nz = pp.noise;
-      nz.step = pp.noise.step + (uint64_t)st;
-      nz.dt = prm->dt;
-      if (pp.kind == RIAB_CELLS_FFL) {
-        // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
-        // previous step's: before the first step, the row the caller passed
-        riab_ffl_cells fc = *(const riab_ffl_cells*)pp.cells;
-        for (int i = 0; i < fc.n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
-          riab_ffl_input& in = fc.inputs[i];
-          if (in.population < 0 || in.population >= n_pops || (in.lag == 0) != (in.population < p) || in.lag < 0 || in.lag > 1)
-            return fail(RIAB_ERR_INVALID, "population %d: FeedForwardLayer input %d (population %d, lag %d) out of order", p, i,
-                        in.population, in.lag);
-          const riab_population& ip = pops[in.population];
-          if (in.lag == 1 && st == 0) continue;
-          if (in.lag == 1 && ip.ring_rows < 2)
-            return fail(RIAB_ERR_INVALID, "population %d feeds a FeedForwardLayer with one step of lag: it needs 2 ring rows", in.population);
-          in.rows_dev = ip.rates_ring + (size_t)((ip.ring_next + st - in.lag) % ip.ring_rows) * A * ip.out.ld;
-          in.ld = ip.out.ld;
-        }
-        rc = riab_neurons_update(agents, env, pp.kind, &fc, &nz, &ro, stream);
-      } else if (p == 0 && src != nullptr) rc = riab_neurons_update(agents, env, pp.kind, pp.cells, &nz, &ro, stream);
-      else if (p == 0 && !skew) rc = riab_step_fused(agents, env, prm, &sio, pp.kind, pp.cells, &nz, &ro, stream);
-      else if (p == 0 && st + 1 < n_steps) {
-        const riab_step_io nxt = step_io(st + 1);          // the motion it runs belongs to step st+1
-        rc = neurons_update_impl<2>(agents, env, prm, &nxt, pp.kind, pp.cells, &nz, &ro, stream);
-      } else rc = riab_neurons_update(agents, env, pp.kind, pp.cells, &nz, &ro, stream);
-      if (rc) return rc;
-    }
-  }
-  return 0;
-}
 
-extern "C" {
 
 int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
              const riab_population* pops, int32_t n_pops, const riab_agent_history* hist, int64_t n_steps,
@@ -2725,30 +2748,6 @@ int riab_step_fused_host(const riab_agents* agents, const riab_env* env, const r
   if (pos_out_host != nullptr) RIAB_CUDA_OK(cudaMemcpyAsync(pos_out_host, agents->pos, bytes, cudaMemcpyDeviceToHost, s));
   return 0;
 }
-
-
-// ---- host-buffer motion step on two streams (see include/riab_b200.h)
-namespace {
-struct HostIo {
-  cudaStream_t side = nullptr;
-  cudaEvent_t up_done = nullptr, motion_done = nullptr, pos_done = nullptr;
-  bool pos_inflight = false;
-};
-thread_local HostIo g_hostio[16];
-int hostio(HostIo*& h) {
-  int dev = 0;
-  RIAB_CUDA_OK(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 16) return fail(RIAB_ERR_UNSUPPORTED, "device ordinal %d", dev);
-  h = &g_hostio[dev];
-  if (h->side == nullptr) {
-    RIAB_CUDA_OK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->up_done, cudaEventDisableTiming));
-    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->motion_done, cudaEventDisableTiming));
-    RIAB_CUDA_OK(cudaEventCreateWithFlags(&h->pos_done, cudaEventDisableTiming));
-  }
-  return 0;
-}
-}  // namespace
 
 int riab_positions_fence(void* stream) {
   HostIo* h = nullptr;
