@@ -331,7 +331,7 @@ typedef struct {
  * (motion -> rates [-> noise] [-> spikes] -> history row).  `cells_kind` selects
  * which of pc / gc / bvc / ovc is read. */
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
-               RIAB_CELLS_FFL = 4 } riab_cells_kind;
+               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
   int64_t ld;
@@ -358,6 +358,34 @@ int riab_neurons_update(const riab_agents* agents, const riab_env* env, int32_t 
 int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
                    const riab_rates_out* out, void* stream);
 
+/* ------------------------------------------------------- RandomSpatialNeurons
+ * Neurons.py:2865-2954: rate[a, i] = sum_j k(pos_a, X_j) targets[j, i] / sum_j k(pos_a, X_j), k = exp(-d^2 / 2 l^2) with
+ * the population's wall_geometry distance d.  k(pos, X) is a PlaceCells row (centres X, widths l, gaussian, [0, 1]);
+ * the contraction with the targets is the FeedForwardLayer GEMM with its A operand generated in registers. */
+typedef struct {
+  riab_place_cells points;   /* the sample points: riab_place_pack block of X in the packed K order (riab_rsn_pack);
+                                packed_dev / centres_dev (k_pad,2 f64, riab_rsn_pack's centres_out) set by the caller */
+  const float* targets_dev;  /* T_hi | T_lo: riab_ffl_pack of targets.T, (n_pad8, k_pad) each */
+  int32_t n_cells;           /* n */
+  int32_t n_points;          /* |X| */
+  int32_t k_pad;             /* filled by riab_rsn_pack: |X| rounded up to 32 */
+  float min_fr, max_fr;      /* the targets' range (validation only: the targets are already scaled) */
+  int32_t reserved;
+} riab_rsn_cells;
+/* Floats of the packed block: the sample-point block (riab_place_pack_floats(k_pad, n_inner_walls)) followed by the
+ * targets block (riab_ffl_pack_floats(n_cells, n_points)); the targets block starts 16-byte aligned. */
+int64_t riab_rsn_pack_floats(int32_t n_cells, int32_t n_points, int32_t n_inner_walls);
+/* X (n_points,2) f64, targets (n_points, n_cells) f64 row-major, lengthscale l.  Packed position p of K stage s (32 points)
+ * holds sample point s*32 + rsn_k(p % 32) so that a consumer thread's 8 fragment columns are 2 runs of 4 packed points;
+ * positions past n_points repeat point 0 and are masked in the kernel.  centres_out: (k_pad,2) f64 in packed order. */
+int riab_rsn_pack(const double* X_host, int32_t n_points, const double* targets_host, int32_t n_cells, double lengthscale,
+                  const double* walls_host, int32_t n_walls, int32_t n_boundary_walls, const double* extent,
+                  int32_t wall_geometry, riab_rsn_cells* meta_out, float* out_host, double* centres_out);
+/* RandomSpatialNeurons.get_state(evaluate_at=None, pos=P): pos_dev (n_pos,2) f64 -> out_dev (n_pos, ld_out) f32; rows
+ * whose x is NaN get zeros.  With RIAB_CELLS_RSN, riab_neurons_update / riab_step_fused / riab_run run the same kernel. */
+int riab_rsn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_rsn_cells* rsn, float* out_dev,
+                   int64_t ld_out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
@@ -367,7 +395,8 @@ int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_
  * History rows go to device rings: row (next + s) % rows for step s. */
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
-  const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* */
+  const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
+                                   riab_rsn_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

@@ -979,3 +979,100 @@ class FeedForwardLayer(Neurons):
             return out[:, : self.n]
         r = out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
         return r[:, 0] if (evaluate_at == "last" and n_pos == 1) else r
+
+
+# =============================================================================
+class RandomSpatialNeurons(Neurons):
+    """ratinabox.RandomSpatialNeurons (Neurons.py:2865-2954): smooth random spatial tunings drawn from a Gaussian process.
+
+    Set-up (host, float64, the reference's global NumPy draws in the reference's order): the sample grid ``X`` =
+    ``discretise_environment(dx=min(0.05, lengthscale))``, its covariance ``Q = kernel(X, X)`` with the population's
+    ``wall_geometry`` distances, and ``targets`` = sigmoid(multivariate_normal(0, Q, size=n).T) in [min_fr, max_fr].
+    ``targets`` is a float64 (|X|, n) array the user may edit; it is re-packed when its bytes change.
+
+    Rates: the kernel-weighted average of the targets, ``k(pos, X) @ targets / sum k(pos, X)``, evaluated in one fused
+    kernel (csrc/riab_rsn.cuh): the kernel row is generated in registers as a PlaceCells row over X and contracted with
+    the targets on the tensor cores.  NaN positions give zero rates."""
+    default_params = {                                              # ratinabox/Neurons.py:2875-2881
+        "lengthscale": 0.1,
+        "max_fr": 1,
+        "min_fr": 0,
+        "n": 10,
+        "wall_geometry": "geodesic",
+        "name": "RandomSpatialNeurons",
+    }
+    _cells_kind = _lib.CELLS_RSN
+
+    def __init__(self, Agent, params={}):
+        super().__init__(Agent, params)
+        self._set_up()
+
+    def _set_up(self):
+        """The host set-up of Neurons.py:2890-2913 (no device work)."""
+        env = self.Agent.Environment
+        if self.wall_geometry == "geodesic" and len(env.walls) > 5:    # Neurons.py:2890-2894
+            print("Geodesic wall geometry only possible in environments with one or no additional walls. Using "
+                  "'line_of_sight' instead. If this is slow, consider trying 'euclidean'")
+            self.wall_geometry = "line_of_sight"
+        assert self.lengthscale >= 0.02, "lengthscale must be greater than 0.02 m"
+        self._effective_geometry()                                   # the device path's limits, before any draw
+        X = env.discretise_environment(dx=min(0.05, self.lengthscale))
+        self.X = X.reshape(-1, X.shape[-1])
+        self.Q = self.kernel(self.X, self.X)
+        with warnings.catch_warnings():                              # Neurons.py:2909-2911
+            warnings.simplefilter("ignore", category=RuntimeWarning)
+            targets = np.random.multivariate_normal(mean=np.zeros(self.Q.shape[0]), cov=self.Q, size=self.n).T
+        from .utils import sigmoid
+        self.targets = sigmoid(targets, max_fr=self.max_fr, min_fr=self.min_fr, mid_x=0, width_x=2)
+
+    def kernel(self, x1, x2):
+        """(len(x1), len(x2)) squared-exponential covariance over the environment's distances (Neurons.py:2944-2954),
+        host float64, with the reference's jitter draws for the wall tests."""
+        from .utils import get_distances_between___accounting_for_environment
+        d = get_distances_between___accounting_for_environment(self.Agent.Environment, x1, x2, self.wall_geometry)
+        return np.exp(-(d ** 2) / (2 * self.lengthscale ** 2))
+
+    def _effective_geometry(self):
+        """The device path's wall geometry: PlaceCells' limits (geodesic only in the box, at most PLACE_MAX_WI inner
+        walls); without inner walls every geometry is the plain distance.  Periodic boundaries are refused by kernel()."""
+        geom = PlaceCells._effective_geometry(self)
+        n_inner = len(self.Agent.Environment.walls) - self.Agent.Environment.los_skip
+        if geom != "euclidean" and n_inner > _lib.PLACE_MAX_WI:
+            raise NotImplementedError(f"at most {_lib.PLACE_MAX_WI} inner walls with {geom} wall geometry on the CUDA path")
+        return geom
+
+    def _signature(self):
+        env = self.Agent.Environment
+        return (np.ascontiguousarray(self.targets, dtype=np.float64).tobytes(),
+                np.ascontiguousarray(self.X, dtype=np.float64).tobytes(), float(self.lengthscale), self.wall_geometry,
+                env._walls_signature(), float(self.min_fr), float(self.max_fr))
+
+    def _pack(self):
+        env = self.Agent.Environment
+        X = np.ascontiguousarray(self.X, dtype=np.float64).reshape(-1, 2)
+        T = np.ascontiguousarray(self.targets, dtype=np.float64)
+        assert T.ndim == 2 and T.shape[0] == X.shape[0], f"targets must have shape ({X.shape[0]}, n)"
+        self.n = T.shape[1]
+        geom = _lib.WALL_GEOMETRIES[self._effective_geometry()]
+        walls = np.ascontiguousarray(env.walls, dtype=np.float64)
+        n_inner = 0 if geom == 0 else walls.shape[0] - env.los_skip
+        c = _lib.RsnCells()
+        host = np.zeros(self._lib.riab_rsn_pack_floats(self.n, X.shape[0], n_inner), dtype=np.float32)
+        k_pad = (X.shape[0] + 31) // 32 * 32
+        centres = np.zeros((k_pad, 2), dtype=np.float64)
+        ext = np.ascontiguousarray(env.extent, dtype=np.float64)
+        _lib.check(self._lib.riab_rsn_pack(_f64p(X), X.shape[0], _f64p(T), self.n, float(self.lengthscale), _f64p(walls),
+                                           walls.shape[0], env.los_skip, _f64p(ext), geom, C.byref(c),
+                                           host.ctypes.data_as(_lib.c_float_p), _f64p(centres)))
+        self._packed = self._upload(host)
+        self._centres_dev = self._upload(centres)
+        point_floats = self._lib.riab_place_pack_floats(k_pad, c.points.n_inner_walls)
+        c.points.packed_dev, c.points.centres_dev = self._packed.data_ptr(), self._centres_dev.data_ptr()
+        c.targets_dev = self._packed.data_ptr() + 4 * point_floats
+        c.min_fr, c.max_fr = float(self.min_fr), float(self.max_fr)
+        return c
+
+    def _rates_from_positions(self, pos_dev, n_pos, out):
+        ag = self.Agent
+        _lib.check(self._lib.riab_rsn_rates(pos_dev.data_ptr(), n_pos, C.byref(ag._env_struct()), C.byref(self._cells()),
+                                            out.data_ptr(), out.stride(0), ag._stream()))

@@ -11,7 +11,7 @@ verbose = False
 from .Environment import Environment          # noqa: E402
 from .Agent import Agent                      # noqa: E402
 from .Neurons import (Neurons, PlaceCells, GridCells, BoundaryVectorCells, FieldOfViewBVCs,   # noqa: E402
-                      ObjectVectorCells, FieldOfViewOVCs, FeedForwardLayer)
+                      ObjectVectorCells, FieldOfViewOVCs, FeedForwardLayer, RandomSpatialNeurons)
 
 __all__ = ["Environment", "Agent", "Neurons", "PlaceCells", "GridCells", "BoundaryVectorCells", "FieldOfViewBVCs",
-           "ObjectVectorCells", "FieldOfViewOVCs", "FeedForwardLayer"]
+           "ObjectVectorCells", "FieldOfViewOVCs", "FeedForwardLayer", "RandomSpatialNeurons"]

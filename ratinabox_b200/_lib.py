@@ -99,6 +99,11 @@ class FflCells(C.Structure):
                 ("inputs", FflInput * FFL_MAX_INPUTS)]
 
 
+class RsnCells(C.Structure):
+    _fields_ = [("points", PlaceCells), ("targets_dev", C.c_void_p), ("n_cells", C.c_int32), ("n_points", C.c_int32),
+                ("k_pad", C.c_int32), ("min_fr", C.c_float), ("max_fr", C.c_float), ("reserved", C.c_int32)]
+
+
 class HistoryView(C.Structure):
     _fields_ = [("agent_ring", C.c_void_p), ("agent_ring_rows", C.c_int32), ("agent_row0", C.c_int32),
                 ("rates_ring", C.c_void_p), ("rates_ring_rows", C.c_int32), ("rates_row0", C.c_int32),
@@ -129,7 +134,8 @@ class AgentHistory(C.Structure):
 PC_DESCRIPTIONS = {"gaussian": 0, "gaussian_threshold": 1, "diff_of_gaussians": 2, "top_hat": 3, "one_hot": 4}
 WALL_GEOMETRIES = {"euclidean": 0, "line_of_sight": 1, "geodesic": 2}
 GC_DESCRIPTIONS = {"rectified_cosines": 0, "shifted_cosines": 1}
-CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL = 0, 1, 2, 3, 4
+CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL, CELLS_RSN = 0, 1, 2, 3, 4, 5
+PLACE_MAX_WI = 8                                              # inner walls of the line-of-sight / geodesic kernels
 ACTIVATIONS = {"linear": 0, "sigmoid": 1, "relu": 2, "tanh": 3, "retanh": 4, "softmax": 5}   # riab_activation
 MAX_REC_ITERS = 4
 
@@ -167,6 +173,10 @@ SYMBOLS = {
     "riab_ffl_pack": (C.c_int, [c_double_p, C.c_int32, C.c_int32, C.POINTER(FflInput), c_float_p]),
     "riab_ffl_rates": (C.c_int, [C.POINTER(FflCells), C.c_int64, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut),
                                  C.c_void_p]),
+    "riab_rsn_pack_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
+    "riab_rsn_pack": (C.c_int, [c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_double, c_double_p, C.c_int32, C.c_int32,
+                                c_double_p, C.c_int32, C.POINTER(RsnCells), c_float_p, c_double_p]),
+    "riab_rsn_rates": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(Env), C.POINTER(RsnCells), C.c_void_p, C.c_int64, C.c_void_p]),
     "riab_step_fused": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                   C.c_int32, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut), C.c_void_p]),
     "riab_neurons_update": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.c_int32, C.c_void_p, C.POINTER(NeuronNoise),

@@ -26,6 +26,7 @@
 #include "riab_grid.cuh"
 #include "riab_motion.cuh"
 #include "riab_place.cuh"
+#include "riab_rsn.cuh"
 #include "riab_traj.cuh"
 
 using namespace riab;
@@ -1915,6 +1916,79 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
   return 0;
 }
 
+// ---------------------------------------------------------------------------
+// RandomSpatialNeurons (riab_rsn.cuh).  The sample points are a place-cell population: make_place validates them and
+// sets up their constants, in the direct (not expanded) Gaussian form with the [0, 1] scale.
+int make_rsn(const riab_rsn_cells* r, const EnvK& env, PlaceConst& c) {
+  if (r == nullptr || r->targets_dev == nullptr) return fail(RIAB_ERR_INVALID, "rsn / targets_dev NULL");
+  if (r->n_cells <= 0 || r->n_points <= 0 || r->k_pad != (r->n_points + FFL_BK - 1) / FFL_BK * FFL_BK ||
+      r->points.n_cells != r->k_pad || r->points.description != RIAB_PC_GAUSSIAN || r->points.min_fr != 0.f ||
+      r->points.max_fr != 1.f)
+    return fail(RIAB_ERR_INVALID, "rsn: bad sizes / sample points (pack with riab_rsn_pack)");
+  if (!(r->min_fr <= r->max_fr)) return fail(RIAB_ERR_INVALID, "rsn: min_fr > max_fr");
+  if (((uintptr_t)r->targets_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "rsn: targets_dev must be 16-byte aligned");
+  int rc;
+  if ((rc = make_place(&r->points, env, c))) return rc;
+  if (r->points.wall_geometry != RIAB_GEOM_EUCLIDEAN && r->points.centres_dev == nullptr)
+    return fail(RIAB_ERR_INVALID, "rsn: centres_dev NULL");
+  c.expanded = 0; c.fold = 0; c.lspan = 0.f; c.kx = 0.f;
+  return 0;
+}
+
+template <int WI, int DESC, int BN>
+int launch_rsn_k(RsnK& k, cudaStream_t s) {
+  constexpr int smem = rsn_smem_bytes<BN>(), CWG = WI >= 4 ? 1 : 2;     // consumer warpgroups (see riab_rsn.cuh)
+  RIAB_CUDA_OK(cudaFuncSetAttribute(k_rsn<WI, DESC, BN, CWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const long long m_tiles = (k.n_rows + 64 * CWG - 1) / (64 * CWG);
+  k.n_tiles = (k.n_cells + BN - 1) / BN;
+  k_rsn<WI, DESC, BN, CWG><<<(unsigned)(m_tiles * k.n_tiles), rsn_threads<CWG>(), smem, s>>>(k);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// the N tile of k_ffl (8, 32 or 64 from n); 8 inner walls stop at 32, whose accumulators fit next to their point registers
+template <int WI, int DESC>
+int launch_rsn_bn(RsnK& k, cudaStream_t s) {
+  if (k.n_cells <= 8) return launch_rsn_k<WI, DESC, 8>(k, s);
+  if (k.n_cells <= 32 || WI >= 8) return launch_rsn_k<WI, DESC, 32>(k, s);
+  if constexpr (WI < 8) return launch_rsn_k<WI, DESC, 64>(k, s);
+  return 0;
+}
+
+// One RandomSpatialNeurons evaluation at n_rows positions (+ noise / spikes through the k_finish_rows post-pass, as for
+// FeedForwardLayers); r and pc checked by make_rsn.
+int launch_rsn(const riab_rsn_cells* r, const PlaceConst& pc, const EnvK& env, const double* pos, long long n_rows,
+               const OutK& out, cudaStream_t s) {
+  if (n_rows == 0) return 0;
+  const int wi = pc.n_inner;
+  const int bn = r->n_cells <= 8 ? 8 : ((r->n_cells <= 32 || wi > 4) ? 32 : 64);    // as launch_rsn_bn
+  const int n_pad = (r->n_cells + 7) / 8 * 8;
+  RsnK k;
+  memset(&k, 0, sizeof(k));
+  int rc;
+  if ((rc = ffl_tmap(&k.thi, r->targets_dev, r->k_pad, n_pad, r->k_pad, bn)) ||
+      (rc = ffl_tmap(&k.tlo, r->targets_dev + (size_t)n_pad * r->k_pad, r->k_pad, n_pad, r->k_pad, bn))) return rc;
+  k.pc = pc;
+  k.walls = env.walls;
+  k.n_cells = r->n_cells; k.ktiles = r->k_pad / FFL_BK; k.n_points = r->n_points;
+  k.n_rows = n_rows; k.ld = out.ld; k.rates = out.rates; k.pos = pos;
+  // the geodesic detour needs the run-time profile switch of place_rates4 (as launch_place), and then has one inner wall
+  if (pc.geometry == RIAB_GEOM_GEODESIC && wi == 1) rc = launch_rsn_bn<1, -1>(k, s);
+  else if (wi == 0) rc = launch_rsn_bn<0, RIAB_PC_GAUSSIAN>(k, s);
+  else if (wi == 1) rc = launch_rsn_bn<1, RIAB_PC_GAUSSIAN>(k, s);
+  else if (wi == 2) rc = launch_rsn_bn<2, RIAB_PC_GAUSSIAN>(k, s);
+  else if (wi <= 4) rc = launch_rsn_bn<4, RIAB_PC_GAUSSIAN>(k, s);
+  else rc = launch_rsn_bn<8, RIAB_PC_GAUSSIAN>(k, s);
+  if (rc) return rc;
+  if (out.noise != nullptr || out.spikes != nullptr) {
+    const int np128 = (r->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
+    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, r->n_cells, np128, n_rows);
+    g_launches++;
+    RIAB_CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
 
 int make_src(const riab_motion_source* src, long long n_agents, SrcK& k) {
   memset(&k, 0, sizeof(k));
@@ -1950,6 +2024,7 @@ struct Pop {
   PlaceConst place; GridConst grid; OvcConst ovc;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
+  const riab_rsn_cells* rsn = nullptr;  // its sample points: `place`
 };
 
 int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* out, const riab_neuron_noise* noise,
@@ -1976,6 +2051,10 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   } else if (kind == RIAB_CELLS_FFL) {
     d.ffl = (const riab_ffl_cells*)cells;
     d.n_cells = d.ffl->n_cells;
+  } else if (kind == RIAB_CELLS_RSN) {
+    d.rsn = (const riab_rsn_cells*)cells;
+    rc = make_rsn(d.rsn, ek, d.place);
+    d.n_cells = d.rsn->n_cells;
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
@@ -1985,7 +2064,8 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
 }
 
 // One population's kernels for one step.  MODE 0: rates at the agents' positions; 1: the motion step fused in; 2: skewed
-// (rates at the current positions while the motion of the next step runs, riab_run).  BVC and FFL populations run MODE 0.
+// (rates at the current positions while the motion of the next step runs, riab_run).  BVC, FFL and RSN populations run
+// MODE 0.
 template <int MODE>
 int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const Pop& d,
                cudaStream_t s, BvcPipe* pipe = nullptr) {
@@ -1996,6 +2076,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
   if constexpr (MODE == 0) {
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
+    if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, ag.n_agents, d.out, s);
     return launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
   } else {
     return fail(RIAB_ERR_INVALID, "cells kind %d is launched unfused", d.kind);
@@ -2004,9 +2085,11 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
 
 // The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), one_hot (an
 // arg-min across cells), BVC (the latency-bound ray kernel wants all its CTAs in ONE wave: the 128-register motion code
-// would halve its occupancy) and FeedForwardLayers (they read other populations' rows, not the positions).
+// would halve its occupancy), FeedForwardLayers (they read other populations' rows, not the positions) and
+// RandomSpatialNeurons (a GEMM kernel without motion warps).
 bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
   return io.collision_mask || io.first_hit || io.n_iters || d.kind == RIAB_CELLS_BVC || d.kind == RIAB_CELLS_FFL ||
+         d.kind == RIAB_CELLS_RSN ||
          (d.kind == RIAB_CELLS_PLACE && d.place.desc == RIAB_PC_ONE_HOT);
 }
 
@@ -2167,7 +2250,8 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   // evaluates rates(s) of the current positions while its producer warps already run motion(s+1); the last step is rates
   // only.  Same results as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source
   // keeps the plain schedule (its motion kernel is cheap next to the rates).
-  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && !onehot0 && !any_ffl && io.xi == nullptr &&
+  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && pops[0].kind != RIAB_CELLS_RSN && !onehot0 && !any_ffl &&
+                    io.xi == nullptr &&
                     !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr;
   plan.sched = skew ? RunPlan::SKEWED : RunPlan::PLAIN;
   plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || pops[0].kind == RIAB_CELLS_FFL);
@@ -2696,6 +2780,55 @@ int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_
   if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
       (rc = check_ffl(ffl, ok, n_rows))) return rc;
   return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------- RandomSpatialNeurons
+int64_t riab_rsn_pack_floats(int32_t n_cells, int32_t n_points, int32_t n_inner_walls) {
+  if (n_cells <= 0 || n_points <= 0) return 0;
+  return riab_place_pack_floats(ffl_k_pad(n_points), n_inner_walls) + riab_ffl_pack_floats(n_cells, n_points);
+}
+
+int riab_rsn_pack(const double* X, int32_t n_points, const double* targets, int32_t n_cells, double lengthscale,
+                  const double* walls, int32_t n_walls, int32_t n_boundary, const double* extent, int32_t geometry,
+                  riab_rsn_cells* meta, float* out, double* centres_out) {
+  if (!X || !targets || !extent || !meta || !out || !centres_out || n_points <= 0 || n_cells <= 0 || !(lengthscale > 0.0))
+    return fail(RIAB_ERR_INVALID, "riab_rsn_pack: bad argument");
+  const int kp = ffl_k_pad(n_points);
+  // the sample points in the packed K order (pads repeat point 0: inside the box, they leave the screen's bounds as they are)
+  std::vector<double> widths((size_t)kp, lengthscale);
+  for (int p = 0; p < kp; ++p) {
+    const int j = (p / FFL_BK) * FFL_BK + rsn_k_of_packed(p % FFL_BK);
+    const int src = j < n_points ? j : 0;
+    centres_out[2 * p] = X[2 * src];
+    centres_out[2 * p + 1] = X[2 * src + 1];
+  }
+  memset(&meta->points, 0, sizeof(meta->points));
+  int rc;
+  if ((rc = riab_place_pack(centres_out, widths.data(), kp, walls, n_walls, n_boundary, extent, geometry, &meta->points, out)))
+    return rc;
+  meta->points.n_cells = kp;
+  meta->points.description = RIAB_PC_GAUSSIAN;
+  meta->points.wall_geometry = geometry;
+  meta->points.min_fr = 0.f;
+  meta->points.max_fr = 1.f;
+  meta->points.top_hat_width = lengthscale;
+  // the targets along K in sample-point order: W = targets.T (n_cells, n_points)
+  std::vector<double> wt((size_t)n_cells * n_points);
+  for (int j = 0; j < n_points; ++j)
+    for (int i = 0; i < n_cells; ++i) wt[(size_t)i * n_points + j] = targets[(size_t)j * n_cells + i];
+  riab_ffl_input tm;
+  if ((rc = riab_ffl_pack(wt.data(), n_cells, n_points, &tm, out + riab_place_pack_floats(kp, meta->points.n_inner_walls))))
+    return rc;
+  meta->targets_dev = nullptr;
+  meta->n_cells = n_cells;
+  meta->n_points = n_points;
+  meta->k_pad = tm.k_pad;
+  return 0;
+}
+
+int riab_rsn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_rsn_cells* rsn, float* out_dev,
+                   int64_t ld_out, void* stream) {
+  return rates_at(RIAB_CELLS_RSN, rsn, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ----------------------------------------------------------------- fused step

@@ -122,3 +122,77 @@ def bin_data_for_histogramming(data, extent, dx, weights=None, norm_by_bincount=
     if return_zero_bins:
         return (heatmap, zero_bins.T[::-1, :])
     return heatmap
+
+
+# ------------------------------------------------------------------------------------------------- environment geometry
+# Host float64 restatements of the reference's pairwise-distance helpers, for set-up computations that must consume the
+# same global NumPy draws as the reference (RandomSpatialNeurons' covariance): same operations, same order, same draws.
+def vector_intercepts(vector_list_a, vector_list_b, return_collisions=False):
+    """utils.vector_intercepts (utils.py:30-118): the intersection parameters (l_a, l_b) of every pair of segments
+    a (N_a,2,2) and b (N_b,2,2) -> (N_a,N_b,2), or with ``return_collisions`` the mask 0 < l_a, l_b < 1.  Both lists
+    are jittered by N(0, 1e-9) draws first, a's then b's, like the reference."""
+    a = np.asarray(vector_list_a, dtype=float).reshape(-1, 2, 2)
+    b = np.asarray(vector_list_b, dtype=float).reshape(-1, 2, 2)
+    a = a + np.random.normal(scale=1e-9, size=a.shape)
+    b = b + np.random.normal(scale=1e-9, size=b.shape)
+    d0 = b[None, :, 0, :] - a[:, None, 0, :]                  # (N_a,N_b,2)
+    sa = (a[:, 1, :] - a[:, 0, :])[:, None, :]
+    sb = (b[:, 1, :] - b[:, 0, :])[None, :, :]
+    sa_px, sa_py = -sa[..., 1], sa[..., 0]                    # [x,y]_p = [-y,x]
+    sb_px, sb_py = -sb[..., 1], sb[..., 0]
+    with np.errstate(divide="ignore", invalid="ignore"):     # parallel segments: inf / nan, never inside (0, 1)
+        l_a = (d0[..., 0] * sb_px + d0[..., 1] * sb_py) / (sa[..., 0] * sb_px + sa[..., 1] * sb_py)
+        l_b = ((-d0[..., 0]) * sa_px + (-d0[..., 1]) * sa_py) / (sb[..., 0] * sa_px + sb[..., 1] * sa_py)
+    if return_collisions:
+        return (l_a > 0) & (l_a < 1) & (l_b > 0) & (l_b < 1)
+    return np.stack((l_a, l_b), axis=-1)
+
+
+def get_distances_between___accounting_for_environment(env, pos1, pos2, wall_geometry="euclidean"):
+    """Environment.get_distances_between___accounting_for_environment (Environment.py:677-779), 2D: (N,M) distances
+    from pos1 (N,2) to pos2 (M,2).  Periodic boundaries wrap the difference vectors; line_of_sight sets the distance of
+    pairs whose segment crosses one of ``walls[4:]`` to 1000; geodesic (at most one wall after the first four) replaces
+    a blocked distance by the shortest detour via an end of that wall that lies inside the environment."""
+    pos1 = np.asarray(pos1, dtype=float).reshape(-1, 2)
+    pos2 = np.asarray(pos2, dtype=float).reshape(-1, 2)
+    vectors = pos1[:, None, :] - pos2[None, :, :]
+    if env.boundary_conditions == "periodic":
+        flip = np.abs(vectors) > (env.scale / 2)
+        vectors[flip] = -np.sign(vectors[flip]) * (env.scale - np.abs(vectors[flip]))
+    distances = np.linalg.norm(vectors, axis=-1)
+    if wall_geometry == "euclidean":
+        return distances
+    segments = np.stack((np.broadcast_to(pos1[:, None, :], vectors.shape),
+                         np.broadcast_to(pos2[None, :, :], vectors.shape)), axis=-2).reshape(-1, 2, 2)
+    walls = env.walls
+    if wall_geometry == "line_of_sight":
+        assert env.boundary_conditions == "solid", "line of sight geometry not available for periodic boundary conditions"
+        blocked = vector_intercepts(segments, walls[4:], return_collisions=True)
+        blocked = (blocked.sum(axis=-1) != 0).reshape(distances.shape)
+        distances[blocked] = 1000
+        return distances
+    if wall_geometry == "geodesic":
+        assert env.boundary_conditions == "solid", "geodesic geometry is not available for periodic boundary conditions"
+        assert len(walls) <= 5, ("unfortunately geodesic geometry is only defined in closed rooms with one additional "
+                                 "wall. Try using \"line_of_sight\" or \"euclidean\" instead.")
+        if len(walls) == 4:
+            return distances
+        wall = walls[4]
+        via = []
+        for end in wall:
+            if env.check_if_position_is_in_environment(end):
+                e = end.reshape(1, 2)
+                via.append(np.linalg.norm(pos1[:, None, :] - e[None, :, :], axis=-1)
+                           + np.linalg.norm(e[:, None, :] - pos2[None, :, :], axis=-1))
+        via = np.array(via)
+        blocked = vector_intercepts(segments, np.expand_dims(wall, axis=0), return_collisions=True).reshape(distances.shape)
+        distances[blocked] = np.amin(via, axis=0)[blocked]
+        return distances
+    raise ValueError(f"unknown wall_geometry {wall_geometry!r}")
+
+
+def sigmoid(x, max_fr=1, min_fr=0, mid_x=1, width_x=2):
+    """utils.activate(x, "sigmoid") (utils.py:961-977): (max_fr - min_fr) / (1 + exp(-beta (x - mid_x))) + min_fr with
+    beta = log(19) / (width_x / 2), so that width_x spans the 5 % to 95 % rise."""
+    beta = np.log((1 - 0.05) / 0.05) / (0.5 * width_x)
+    return ((max_fr - min_fr) / (1 + np.exp(-beta * (x - mid_x)))) + min_fr
