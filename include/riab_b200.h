@@ -331,7 +331,7 @@ typedef struct {
  * (motion -> rates [-> noise] [-> spikes] -> history row).  `cells_kind` selects
  * which of pc / gc / bvc / ovc is read. */
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
-               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5 } riab_cells_kind;
+               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
   int64_t ld;
@@ -386,6 +386,43 @@ int riab_rsn_pack(const double* X_host, int32_t n_points, const double* targets_
 int riab_rsn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_rsn_cells* rsn, float* out_dev,
                    int64_t ld_out, void* stream);
 
+/* ------------------------------------------- kinematic cells (RIAB_CELLS_KIN)
+ * HeadDirectionCells (Neurons.py:2357-2485), VelocityCells (:2534-2583) and SpeedCell (:2586-2651): rates from the
+ * agent's head direction, velocity or measured velocity, no position tuning.
+ *   head direction: fr_i = von_mises(get_angle(d), mu_i, sigma_i, norm=1) (max_fr - min_fr) + min_fr      (:2466-2474)
+ *                   d = head_direction, or velocity / |velocity| when use_velocity                        (:2428-2460)
+ *   velocity:       the use_velocity head-direction rates times |velocity| inv_one_sigma_speed             (:2580-2582)
+ *   speed:          |measured_velocity| inv_one_sigma_speed (max_fr - min_fr) + min_fr                     (:2641-2650)
+ * utils.get_angle's 1e-6 eps (utils.py:258-260) is kept; a zero velocity gives NaN like the reference's 0/0. */
+typedef enum { RIAB_KIN_HEAD_DIRECTION = 0, RIAB_KIN_VELOCITY = 1, RIAB_KIN_SPEED = 2 } riab_kin_variant;
+typedef struct {
+  int32_t n_cells;
+  int32_t variant;               /* riab_kin_variant */
+  int32_t use_velocity;          /* head direction: 1 = the normalised velocity replaces it (get_state(use_velocity=True));
+                                    velocity cells: always 1 */
+  int32_t reserved0;
+  float min_fr, max_fr;
+  double inv_one_sigma_speed;    /* 1 / (Agent.speed_mean + Agent.speed_std), taken at construction (:2567, :2625) */
+  const float* packed_dev;       /* riab_kin_pack output */
+  int32_t n_pad;                 /* filled by riab_kin_pack */
+  int32_t reserved1;
+} riab_kin_cells;
+/* Floats of the packed block: cos(mu/2) | sin(mu/2) | k_q = sqrt(2 kappa log2(e)), kappa = 1/sigma^2 (utils.py:452), each
+ * n_pad = n_cells rounded up to 128; pads and speed cells hold (1, 0, 0). */
+int64_t riab_kin_pack_floats(int32_t n_cells);
+/* preferred_angles / angular_tunings (n_cells) f64 radians (Neurons.py:2405-2409; NULL for RIAB_KIN_SPEED); computed in
+ * float64, stored as float32.  Fills every field of cells_out but packed_dev. */
+int riab_kin_pack(const double* preferred_angles, const double* angular_tunings, int32_t n_cells, int32_t variant,
+                  int32_t use_velocity, float min_fr, float max_fr, double one_sigma_speed, riab_kin_cells* cells_out,
+                  float* out_host);
+/* get_state away from the agents' step: vec_dev (n_pos,2) f64 when vec_per_position, else one (2) vector for every row --
+ * the head direction (use_velocity 0), the velocity (use_velocity 1) or, for speed cells, the velocity whose norm is the
+ * speed -> out_dev (n_pos, ld_out) f32.  speed_scale: velocity cells' factor |Agent.velocity| / one_sigma_speed of every
+ * row (Neurons.py:2581); a negative value takes each row's own |vec| inv_one_sigma_speed instead (vec = the agents'
+ * velocities).  No noise, no NaN-position masking (get_state does neither). */
+int riab_kin_rates(const double* vec_dev, int32_t vec_per_position, int64_t n_pos, double speed_scale,
+                   const riab_kin_cells* cells, float* out_dev, int64_t ld_out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
@@ -396,7 +433,7 @@ int riab_rsn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, co
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
-                                   riab_rsn_cells* */
+                                   riab_rsn_cells* / riab_kin_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

@@ -256,6 +256,20 @@ class Neurons:
             return out[:, : self.n]
         return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
 
+    def get_head_direction_averaged_state(self, evaluate_at="agent", angular_resolution_degrees=10, **kwargs):
+        """Neurons.get_head_direction_averaged_state (ratinabox/Neurons.py:176-192): the mean of ``get_state`` over the
+        head directions at ``np.linspace(0, 2 pi, int(360 / angular_resolution_degrees))`` (0 and 2 pi both count), for
+        head-direction-tuned populations (HeadDirectionCells, egocentric vector cells); the others ignore the head
+        direction.  The rates are summed on the device in float64.  Returns (n, n_pos) float64."""
+        kwargs.pop("return_tensor", None)
+        n_angles = int(360 / angular_resolution_degrees)
+        acc = None
+        for ang in np.linspace(0, 2 * np.pi, n_angles):
+            r = self.get_state(evaluate_at=evaluate_at, head_direction=np.array([np.cos(ang), np.sin(ang)]),
+                               return_tensor=True, **kwargs)
+            acc = r.to(self._torch.float64) if acc is None else acc.add_(r)
+        return (acc / n_angles).T.contiguous().cpu().numpy()
+
     # ------------------------------------------------------------------ firingrate
     @property
     def firingrate(self):
@@ -1076,3 +1090,183 @@ class RandomSpatialNeurons(Neurons):
         ag = self.Agent
         _lib.check(self._lib.riab_rsn_rates(pos_dev.data_ptr(), n_pos, C.byref(ag._env_struct()), C.byref(self._cells()),
                                             out.data_ptr(), out.stride(0), ag._stream()))
+
+
+# =============================================================================
+class _KinematicCells(Neurons):
+    """Populations tuned to the agent's motion, not its position (HeadDirectionCells, VelocityCells, SpeedCell): one
+    kernel kind (RIAB_CELLS_KIN, csrc/riab_kin.cuh) whose producer warps read the agent's float64 head direction,
+    velocity or measured velocity."""
+    _cells_kind = _lib.CELLS_KIN
+    _variant = None
+    one_sigma_speed = 1.0
+
+    def _tuning(self):
+        """(preferred_angles, angular_tunings) as float64 arrays, or (None, None) for a speed cell."""
+        return None, None
+
+    def _signature(self):
+        pref, tun = self._tuning()
+        return (None if pref is None else pref.tobytes(), None if tun is None else tun.tobytes(), float(self.min_fr),
+                float(self.max_fr), float(self.one_sigma_speed), self.n)
+
+    def _pack(self):
+        pref, tun = self._tuning()
+        if pref is not None:
+            assert tun.shape == pref.shape, "preferred_angles and angular_tunings must have the same length"
+            self.n = pref.shape[0]
+        c = _lib.KinCells()
+        host = np.zeros(self._lib.riab_kin_pack_floats(self.n), dtype=np.float32)
+        _lib.check(self._lib.riab_kin_pack(None if pref is None else _f64p(pref), None if tun is None else _f64p(tun), self.n,
+                                           self._variant, 0, float(self.min_fr), float(self.max_fr),
+                                           float(self.one_sigma_speed), C.byref(c), host.ctypes.data_as(_lib.c_float_p)))
+        self._packed = self._upload(host)
+        c.packed_dev = self._packed.data_ptr()
+        return c
+
+    def _state(self, evaluate_at, use_velocity, vector=None, speed_scale=-1.0, **kwargs):
+        """Rates at the agents (evaluate_at="agent": every agent's own head direction / velocity / measured velocity) or
+        for the given ``vector``, one (2,) for every position or one per position, over the reference's n_pos: the
+        discretised environment for "all", ``pos``'s rows, else 1 (Neurons.py:2476-2483).  (n, n_pos) float64, or with
+        ``return_tensor=True`` the (n_pos, n) float32 device tensor."""
+        torch = self._torch
+        ag = self.Agent
+        c = _lib.KinCells.from_buffer_copy(self._cells())
+        c.use_velocity = 1 if use_velocity else 0
+        if evaluate_at == "agent":
+            ag._flush_pending()
+            ag._sync_user_writes()
+            vec = ag._s["measured_velocity" if self._variant == _lib.KIN_SPEED else
+                        ("velocity" if use_velocity else "head_direction")]
+            n_pos = ag.n_agents
+        else:
+            if isinstance(vector, torch.Tensor):
+                vec = vector.to(device=self.device, dtype=torch.float64).reshape(-1, 2).contiguous()
+            else:
+                vec = torch.as_tensor(np.array(vector, dtype=np.float64).reshape(-1, 2), device=self.device)
+            if evaluate_at == "all":
+                n_pos = ag.Environment.flattened_discrete_coords.shape[0]
+            elif "pos" in kwargs:
+                n_pos = int(kwargs["pos"].reshape(-1, 2).shape[0]) if isinstance(kwargs["pos"], torch.Tensor) \
+                    else int(np.asarray(kwargs["pos"]).reshape(-1, 2).shape[0])
+            else:
+                n_pos = int(vec.shape[0])
+            if vec.shape[0] not in (1, n_pos):
+                raise ValueError(f"{vec.shape[0]} direction / velocity vectors for {n_pos} positions: pass one (2,) vector "
+                                 "or one per position")
+        per_position = 1 if (evaluate_at == "agent" or vec.shape[0] > 1) else 0
+        out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
+        _lib.check(self._lib.riab_kin_rates(vec.data_ptr(), per_position, n_pos, float(speed_scale), C.byref(c),
+                                            out.data_ptr(), out.stride(0), ag._stream()))
+        if kwargs.get("return_tensor", False):
+            return out[:, : self.n]
+        return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
+
+
+class HeadDirectionCells(_KinematicCells):
+    """ratinabox.HeadDirectionCells (Neurons.py:2357-2485), 2D: cell i fires
+    ``von_mises(get_angle(head_direction), preferred_angles[i], angular_tunings[i], norm=1) * (max_fr - min_fr) + min_fr``.
+    ``preferred_angles`` / ``angular_tunings`` (radians) are float64 arrays the user may edit; they are re-packed when
+    their bytes change.  Away from the agent the ``head_direction`` / ``velocity`` / ``vel`` kwargs take one (2,) vector
+    or one per position."""
+    default_params = {                                              # ratinabox/Neurons.py:2383-2389
+        "min_fr": 0,
+        "max_fr": 1,
+        "n": 10,
+        "angular_spread_degrees": 45,
+        "name": "HeadDirectionCells",
+    }
+    _variant = _lib.KIN_HEAD_DIRECTION
+
+    def __init__(self, Agent, params={}):
+        if Agent.Environment.dimensionality != "2D":
+            raise NotImplementedError("HeadDirectionCells in 1D environments are outside the CUDA hot path")
+        super().__init__(Agent, params)
+        self.preferred_angles = np.linspace(0, 2 * np.pi, self.n + 1)[:-1]           # Neurons.py:2404-2409
+        self.angular_tunings = np.array([self.params["angular_spread_degrees"] * np.pi / 180] * self.n)
+
+    def _tuning(self):
+        return (np.ascontiguousarray(self.preferred_angles, dtype=np.float64).reshape(-1),
+                np.ascontiguousarray(self.angular_tunings, dtype=np.float64).reshape(-1))
+
+    def _direction_kwarg(self, use_velocity, kwargs):
+        """The vector get_state reads away from the agent, with the reference's warning and prints (Neurons.py:2428-2459)."""
+        if not use_velocity:
+            if "head_direction" in kwargs:
+                return kwargs["head_direction"]
+            if "vel" in kwargs:
+                warnings.warn("'vel' kwarg deprecated in favour of 'head_direction'")
+                return kwargs["vel"]
+            print("HeadDirection cells need a head direction but you didn't pass one. Taking ", end="")
+            print("[1,0] as default", end="")
+            print("Recommended to pass one in the 'head_direction' argument of get_state()")
+            return [1, 0]
+        if "velocity" in kwargs:
+            return kwargs["velocity"]
+        print("HeadDirection cells need a velocity but you didn't pass one. Taking ", end="")
+        print("[1,0] as default", end="")
+        print("Recommended to pass one in the 'velocity' argument of get_state()")
+        return [1, 0]
+
+    def get_state(self, evaluate_at="agent", use_velocity=False, **kwargs):
+        """HeadDirectionCells.get_state (Neurons.py:2421-2485): with evaluate_at="agent" every agent's head direction
+        (its normalised velocity with ``use_velocity=True``) -- any head_direction kwarg is ignored there, like the
+        reference -- else the kwargs.  (n, n_pos)."""
+        use_velocity = bool(use_velocity)
+        vector = None if evaluate_at == "agent" else self._direction_kwarg(use_velocity, kwargs)
+        return self._state(evaluate_at, use_velocity, vector, **kwargs)
+
+
+class VelocityCells(HeadDirectionCells):
+    """ratinabox.VelocityCells (Neurons.py:2534-2583): the use_velocity HeadDirectionCells rates times
+    ``|Agent.velocity| / one_sigma_speed``, one_sigma_speed = speed_mean + speed_std at construction.  A zero velocity
+    gives NaN rates like the reference.  Away from the agent the speed factor is the Agent's own velocity, which is one
+    speed only for one agent: with n_agents > 1 that raises ValueError."""
+    default_params = {                                              # ratinabox/Neurons.py:2552-2556
+        "min_fr": 0,
+        "max_fr": 1,
+        "name": "VelocityCells",
+    }
+    _variant = _lib.KIN_VELOCITY
+
+    def __init__(self, Agent, params={}):
+        self.one_sigma_speed = Agent.speed_mean + Agent.speed_std                     # Neurons.py:2567
+        super().__init__(Agent, params)
+
+    def get_state(self, evaluate_at="agent", **kwargs):
+        """VelocityCells.get_state (Neurons.py:2577-2583).  (n, n_pos)."""
+        speed_scale = -1.0                               # at the agents: every agent's own |velocity| / one_sigma_speed
+        if evaluate_at != "agent":
+            if self.Agent.n_agents > 1:
+                raise ValueError("VelocityCells.get_state away from the agent scales the rates by |Agent.velocity|, one "
+                                 "speed per agent: evaluate at the agents, or use an Agent with n_agents=1")
+            speed_scale = np.linalg.norm(self.Agent.velocity) / self.one_sigma_speed
+        vector = None if evaluate_at == "agent" else self._direction_kwarg(True, kwargs)
+        return self._state(evaluate_at, True, vector, speed_scale=speed_scale, **kwargs)
+
+
+class SpeedCell(_KinematicCells):
+    """ratinabox.SpeedCell (Neurons.py:2586-2651): one cell, ``|v| / one_sigma_speed * (max_fr - min_fr) + min_fr`` with
+    v the measured velocity (the history's "vel", Agent.py:517) at the agent, else the ``vel`` kwarg (one (2,) vector, or
+    one per position).  The population is one cell wide from the start (the reference sizes its noise, and so its rows,
+    for the default n = 10 before setting n = 1)."""
+    default_params = {                                              # ratinabox/Neurons.py:2603-2607
+        "min_fr": 0,
+        "max_fr": 1,
+        "name": "SpeedCell",
+    }
+    _variant = _lib.KIN_SPEED
+
+    def __init__(self, Agent, params={}):
+        params = dict(params)
+        n_given = params.get("n", 1)
+        params["n"] = 1
+        super().__init__(Agent, params)
+        if n_given != 1:                                            # Neurons.py:2621-2622
+            warnings.warn(f"Ignoring 'n' parameter value ({n_given}) that was passed for {self.name}. Only 1 speed cell is needed.")
+        self.one_sigma_speed = self.Agent.speed_mean + self.Agent.speed_std           # Neurons.py:2625
+
+    def get_state(self, evaluate_at="agent", **kwargs):
+        """SpeedCell.get_state (Neurons.py:2632-2651).  (1, n_pos) with n_pos as for HeadDirectionCells."""
+        vector = None if evaluate_at == "agent" else kwargs["vel"]
+        return self._state(evaluate_at, False, vector, **kwargs)

@@ -11,7 +11,9 @@ verbose = False
 from .Environment import Environment          # noqa: E402
 from .Agent import Agent                      # noqa: E402
 from .Neurons import (Neurons, PlaceCells, GridCells, BoundaryVectorCells, FieldOfViewBVCs,   # noqa: E402
-                      ObjectVectorCells, FieldOfViewOVCs, FeedForwardLayer, RandomSpatialNeurons)
+                      ObjectVectorCells, FieldOfViewOVCs, FeedForwardLayer, RandomSpatialNeurons,
+                      HeadDirectionCells, VelocityCells, SpeedCell)
 
 __all__ = ["Environment", "Agent", "Neurons", "PlaceCells", "GridCells", "BoundaryVectorCells", "FieldOfViewBVCs",
-           "ObjectVectorCells", "FieldOfViewOVCs", "FeedForwardLayer", "RandomSpatialNeurons"]
+           "ObjectVectorCells", "FieldOfViewOVCs", "FeedForwardLayer", "RandomSpatialNeurons", "HeadDirectionCells",
+           "VelocityCells", "SpeedCell"]

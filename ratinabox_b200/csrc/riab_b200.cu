@@ -4,7 +4,8 @@
 //   k_agent_update      Agent.update, one agent per thread (float64)
 //   k_agent_update_src  Agent.update from an imported trajectory / forced positions, one agent per thread (float64)
 //   k_traj_build        not-a-knot spline of imported trajectories, one thread per (trajectory, axis) column
-//   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells:
+//   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells / ObjectVectorCells /
+//                       head direction, velocity and speed cells:
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
@@ -24,6 +25,7 @@
 #include "riab_ffl.cuh"
 #include "riab_ovc.cuh"
 #include "riab_grid.cuh"
+#include "riab_kin.cuh"
 #include "riab_motion.cuh"
 #include "riab_place.cuh"
 #include "riab_rsn.cuh"
@@ -360,12 +362,13 @@ struct PlacePolicy {
   // Euclidean Gaussian loop is HBM-bound and hides the dense stream's instructions under its stores, the line-of-sight
   // loop with the post-pass needs 8 producer warps and loses next to them.  The dense stream stays.
   static constexpr bool THIN = false;
-  static __device__ __forceinline__ const double* head_dir(const Const&) { return nullptr; }
+  static constexpr bool POSITIONAL = true;
+  static __device__ __forceinline__ void given_dir(const Const&, long long, double&, double&) {}
   static __device__ __forceinline__ void prepare(double* aux, const double* s_walls, const Const& c) {
     place_wall_invariants(aux, s_walls + 4 * c.wall0, WI > 0 ? c.n_inner : 0);
   }
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, const double* s_walls,
-                                                const double* aux, const Const& c, const EnvK& env) {
+  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, double, double, double, double,
+                                                const double* s_walls, const double* aux, const Const& c, const EnvK& env) {
     place_agent_record<WI>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
   }
   static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI>(r, c, cell0); }
@@ -385,10 +388,11 @@ struct GridPolicy {
   static constexpr int REC = 4;
   static constexpr bool LIGHT = false;    // 36 cell registers per thread do not fit StepCfg<8>'s 56-register consumers
   static constexpr bool THIN = true;      // bounded rates, consumer-bound loop: thinned spikes
-  static __device__ __forceinline__ const double* head_dir(const Const&) { return nullptr; }
+  static constexpr bool POSITIONAL = true;
+  static __device__ __forceinline__ void given_dir(const Const&, long long, double&, double&) {}
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, const double*, const double*,
-                                                const Const&, const EnvK& env) {
+  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, double, double, double, double,
+                                                const double*, const double*, const Const&, const EnvK& env) {
     rec[0] = (float)(px - env.cxm);
     rec[1] = (float)(py - env.cym);
   }
@@ -408,10 +412,15 @@ struct OvcPolicy {
   static constexpr int REC = OVC_REC;
   static constexpr bool LIGHT = false;
   static constexpr bool THIN = false;     // sums over objects: no a-priori rate bound
-  static __device__ __forceinline__ const double* head_dir(const Const& c) { return c.head_dir; }
+  static constexpr bool POSITIONAL = true;
+  // egocentric cells evaluated at given positions: their head directions
+  static __device__ __forceinline__ void given_dir(const Const& c, long long i, double& x, double& y) {
+    if (c.head_dir != nullptr) { x = c.head_dir[2 * i]; y = c.head_dir[2 * i + 1]; }
+  }
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double hdx, double hdy,
-                                                const double* s_walls, const double*, const Const& c, const EnvK&) {
+  static __device__ __forceinline__ void record(float* rec, double px, double py, double hdx, double hdy, double, double,
+                                                double, double, const double* s_walls, const double*, const Const& c,
+                                                const EnvK&) {
     ovc_agent_record(rec, px, py, hdx, hdy, s_walls, c);
   }
   static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { ovc_load_cells(r, c, cell0); }
@@ -419,6 +428,34 @@ struct OvcPolicy {
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
                                                 uint32_t, bool&) {
     ovc_rates4(o, r, c, rec);
+  }
+  static __device__ __forceinline__ int expanded(const Const&) { return 0; }
+  static __device__ __forceinline__ int wall0(const Const&) { return 0; }
+};
+
+// Head direction / velocity / speed cells: the record is the agent's kinematic state, not its position.  MODE 0 takes the
+// state from KinConst::vec (the agents' arrays, or get_state's vectors with no positions at all: pos_in may be NULL).
+struct KinPolicy {
+  using Const = KinConst;
+  using Regs = KinCellRegs;
+  static constexpr int REC = KIN_REC;
+  static constexpr bool LIGHT = true;     // one ex2 per rate, 12 cell registers: HBM-bound consumers
+  static constexpr bool THIN = false;     // velocity and speed rates have no a-priori bound: dense spike stream
+  static constexpr bool POSITIONAL = false;
+  static __device__ __forceinline__ void given_dir(const Const& c, long long i, double& x, double& y) {
+    if (c.vec != nullptr) { x = c.vec[c.vec_ld * i]; y = c.vec[c.vec_ld * i + 1]; }
+  }
+  static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
+  static __device__ __forceinline__ void record(float* rec, double, double, double hdx, double hdy, double vx, double vy,
+                                                double mvx, double mvy, const double*, const double*, const Const& c,
+                                                const EnvK&) {
+    kin_agent_record(rec, hdx, hdy, vx, vy, mvx, mvy, c);
+  }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { kin_load_cells(r, c, cell0); }
+  template <bool DEFER, int EXP = -1>
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
+                                                uint32_t, bool&) {
+    kin_rates4(o, r, c, rec);
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const&) { return 0; }
@@ -924,7 +961,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             if constexpr (MODE == 4) agent_update_src_one(ag, mp, md, io_st, run.src, t_st, env, a0 + lane, as);
             else agent_update_one<false>(ag, mp, md, io_st, env, s_walls, a0 + lane, as);
             nanpos = (as.px != as.px);
-            P::record(s_slot[s].rec[lane], as.px, as.py, as.hdx, as.hdy, s_walls, s_aux, pc, env);
+            P::record(s_slot[s].rec[lane], as.px, as.py, as.hdx, as.hdy, as.vx, as.vy, as.mvx, as.mvy, s_walls, s_aux, pc, env);
           }
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
         }
@@ -947,7 +984,8 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             const long long i = a0 + lane;
             const double px = ag.pos[2 * i], py = ag.pos[2 * i + 1];
             nanpos = (px != px);
-            P::record(s_slot[s].rec[lane], px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], s_walls, s_aux, pc, env);
+            P::record(s_slot[s].rec[lane], px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], ag.velocity[2 * i],
+                      ag.velocity[2 * i + 1], ag.measured_velocity[2 * i], ag.measured_velocity[2 * i + 1], s_walls, s_aux, pc, env);
           }
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
           if (lane < na) {
@@ -959,18 +997,18 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
         bool nanpos = false;
         if (lane < na) {
           const long long i = a0 + lane;
-          double px, py, hdx = 1.0, hdy = 0.0;
+          double px = 0.0, py = 0.0, hdx = 1.0, hdy = 0.0, vx, vy, mvx, mvy;
           if (MODE == 1) {
             AgentState st;
             agent_update_one<false>(ag, mp, md, io, env, s_walls, i, st);
-            px = st.px; py = st.py; hdx = st.hdx; hdy = st.hdy;
+            px = st.px; py = st.py; hdx = st.hdx; hdy = st.hdy; vx = st.vx; vy = st.vy; mvx = st.mvx; mvy = st.mvy;
           } else {
-            px = pos_in[2 * i]; py = pos_in[2 * i + 1];
-            const double* hd = P::head_dir(pc);                 // egocentric cells evaluated at given positions
-            if (hd != nullptr) { hdx = hd[2 * i]; hdy = hd[2 * i + 1]; }
+            if (P::POSITIONAL || pos_in != nullptr) { px = pos_in[2 * i]; py = pos_in[2 * i + 1]; }
+            P::given_dir(pc, i, hdx, hdy);                      // the one given vector stands for every kinematic input
+            vx = mvx = hdx; vy = mvy = hdy;
           }
           nanpos = (px != px);
-          P::record(s_slot[s].rec[lane], px, py, hdx, hdy, s_walls, s_aux, pc, env);
+          P::record(s_slot[s].rec[lane], px, py, hdx, hdy, vx, vy, mvx, mvy, s_walls, s_aux, pc, env);
         }
         publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
       }
@@ -1618,6 +1656,25 @@ int make_ovc(const riab_ovc_cells* oc, const EnvK& env, const double* head_dir, 
   return 0;
 }
 
+// Kinematic cells at the agents: the vector their variant reads, one per agent (Neurons.py:2430, :2448, :2642).
+int make_kin(const riab_kin_cells* kc, const riab_agents& ag, KinConst& c) {
+  if (kc == nullptr || kc->packed_dev == nullptr) return fail(RIAB_ERR_INVALID, "kinematic cells / packed_dev NULL");
+  if (kc->variant < RIAB_KIN_HEAD_DIRECTION || kc->variant > RIAB_KIN_SPEED) return fail(RIAB_ERR_INVALID, "bad kinematic variant %d", kc->variant);
+  if (kc->n_cells <= 0 || kc->n_pad != (kc->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD)
+    return fail(RIAB_ERR_INVALID, "kinematic cells: n_cells %d / n_pad %d (pack with riab_kin_pack)", kc->n_cells, kc->n_pad);
+  if (((uintptr_t)kc->packed_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "kinematic cells: packed_dev must be 16-byte aligned");
+  memset(&c, 0, sizeof(c));
+  c.n_cells = kc->n_cells; c.n_pad = kc->n_pad; c.variant = kc->variant;
+  c.use_vel = (kc->variant == RIAB_KIN_VELOCITY || kc->use_velocity) ? 1 : 0;
+  c.min_fr = kc->min_fr; c.span = kc->max_fr - kc->min_fr;
+  c.inv_oss = kc->inv_one_sigma_speed;
+  c.fixed_scale = -1.0;
+  c.packed = kc->packed_dev;
+  c.vec = kc->variant == RIAB_KIN_SPEED ? ag.measured_velocity : (c.use_vel ? ag.velocity : ag.head_direction);
+  c.vec_ld = 2;
+  return 0;
+}
+
 int g_num_sms = 0;
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
@@ -2021,7 +2078,7 @@ struct Pop {
   int kind = -1, n_cells = 0;
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
-  PlaceConst place; GridConst grid; OvcConst ovc;
+  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
   const riab_rsn_cells* rsn = nullptr;  // its sample points: `place`
@@ -2055,6 +2112,9 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
     d.rsn = (const riab_rsn_cells*)cells;
     rc = make_rsn(d.rsn, ek, d.place);
     d.n_cells = d.rsn->n_cells;
+  } else if (kind == RIAB_CELLS_KIN) {
+    rc = make_kin((const riab_kin_cells*)cells, ag, d.kin);
+    d.n_cells = d.kin.n_cells;
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
@@ -2073,6 +2133,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
   if (d.kind == RIAB_CELLS_PLACE) return launch_place<MODE>(ek, ag, mp, io, d.place, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_GRID) return launch_tile<GridPolicy, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
   if constexpr (MODE == 0) {
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
@@ -2246,7 +2307,7 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
   const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
                        ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
-  // Skewed schedule (population 0 is a Place / Grid / OVC population): motion(0) alone, then per step one kernel that
+  // Skewed schedule (population 0 is a Place / Grid / OVC / kinematic population): motion(0) alone, then per step one kernel that
   // evaluates rates(s) of the current positions while its producer warps already run motion(s+1); the last step is rates
   // only.  Same results as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source
   // keeps the plain schedule (its motion kernel is cheap next to the rates).
@@ -2707,6 +2768,50 @@ int riab_bvc_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, co
                    int64_t ld_out, void* stream) {
   return rates_at(RIAB_CELLS_BVC, bvc, pos_dev, n_pos, env, head_direction_dev, scratch_dev, first_wall_dev, out_dev, ld_out,
                   stream);
+}
+
+// ------------------------------------------------------------ kinematic cells
+int64_t riab_kin_pack_floats(int32_t n_cells) { return (int64_t)place_n_pad(n_cells) * 3; }
+
+int riab_kin_pack(const double* preferred_angles, const double* angular_tunings, int32_t n, int32_t variant,
+                  int32_t use_velocity, float min_fr, float max_fr, double one_sigma_speed, riab_kin_cells* meta, float* out) {
+  if (!meta || !out || n <= 0 || variant < RIAB_KIN_HEAD_DIRECTION || variant > RIAB_KIN_SPEED ||
+      (variant != RIAB_KIN_SPEED && (!preferred_angles || !angular_tunings)))
+    return fail(RIAB_ERR_INVALID, "riab_kin_pack: bad argument");
+  const int np = place_n_pad(n);
+  const double log2e = 1.4426950408889634;
+  for (int i = 0; i < np; ++i) {
+    const bool in = i < n && variant != RIAB_KIN_SPEED;
+    const double kappa = in ? 1.0 / (angular_tunings[i] * angular_tunings[i]) : 0.0;   // utils.von_mises (utils.py:452)
+    out[i] = in ? (float)cos(0.5 * preferred_angles[i]) : 1.f;
+    out[(size_t)np + i] = in ? (float)sin(0.5 * preferred_angles[i]) : 0.f;
+    out[(size_t)2 * np + i] = (float)sqrt(2.0 * kappa * log2e);
+  }
+  meta->n_cells = n; meta->variant = variant; meta->use_velocity = (variant == RIAB_KIN_VELOCITY) ? 1 : (use_velocity ? 1 : 0);
+  meta->reserved0 = 0; meta->reserved1 = 0;
+  meta->min_fr = min_fr; meta->max_fr = max_fr;
+  meta->inv_one_sigma_speed = 1.0 / one_sigma_speed;
+  meta->n_pad = np;
+  return 0;
+}
+
+int riab_kin_rates(const double* vec_dev, int32_t vec_per_position, int64_t n_pos, double speed_scale,
+                   const riab_kin_cells* cells, float* out_dev, int64_t ld_out, void* stream) {
+  if (n_pos < 0 || (n_pos > 0 && vec_dev == nullptr)) return fail(RIAB_ERR_INVALID, "riab_kin_rates: bad argument");
+  if (n_pos == 0) return 0;
+  EnvK ek;
+  memset(&ek, 0, sizeof(ek));                       // no walls: the rates do not depend on a position
+  riab_rates_out ro = {};
+  ro.rates_row = out_dev; ro.ld = ld_out;
+  riab_agents at = {};
+  at.n_agents = n_pos;
+  at.head_direction = at.velocity = at.measured_velocity = (double*)vec_dev;
+  Pop d;
+  int rc;
+  if ((rc = make_pop(ek, RIAB_CELLS_KIN, cells, &ro, nullptr, 1.0, at, d))) return rc;
+  d.kin.vec_ld = vec_per_position ? 2 : 0;
+  d.kin.fixed_scale = speed_scale;
+  return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------ ObjectVectorCells
