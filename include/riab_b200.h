@@ -331,7 +331,7 @@ typedef struct {
  * (motion -> rates [-> noise] [-> spikes] -> history row).  `cells_kind` selects
  * which of pc / gc / bvc / ovc is read. */
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
-               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6 } riab_cells_kind;
+               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
   int64_t ld;
@@ -423,6 +423,38 @@ int riab_kin_pack(const double* preferred_angles, const double* angular_tunings,
 int riab_kin_rates(const double* vec_dev, int32_t vec_per_position, int64_t n_pos, double speed_scale,
                    const riab_kin_cells* cells, float* out_dev, int64_t ld_out, void* stream);
 
+/* ------------------------------------------------ AgentVectorCells (RIAB_CELLS_AVC)
+ * AgentVectorCells / FieldOfViewAVCs (Neurons.py:2151-2351): ObjectVectorCells whose single "object" is the position of
+ * another Agent, with no type mask (:2242-2320):
+ *   fr_i = gaussian(d; mu_d_i, sigma_d_i, norm=1) von_mises(bearing; mu_theta_i, sigma_theta_i, norm=1) (max_fr - min_fr) + min_fr
+ *   d       = |pos - partner|, or 1000 when walls_occlude and an inner wall (walls[4:]) crosses the segment (:2235-2247)
+ *   bearing = utils.get_angle(partner - pos) [- utils.get_angle(head_direction) when egocentric]        (:2248-2279)
+ * The agents of a batch are paired row by row: row i sees partner row i, or partner row 0 when n_other == 1. */
+typedef struct {
+  int32_t n_cells;
+  int32_t walls_occlude;         /* 1: wall_geometry "line_of_sight", 0: "euclidean" (:2189-2192) */
+  int32_t egocentric;            /* reference_frame == "egocentric" */
+  int32_t partner_is_self;       /* 1: the Agent is its own partner, each row reads its own (possibly just moved) position */
+  float min_fr, max_fr;
+  const float* packed_dev;       /* device block written by riab_avc_pack (riab_avc_pack_floats floats) */
+  const double* other_pos_dev;   /* the partner's positions (n_other, 2) f64; NULL and partner_is_self == 0: no partner
+                                    (tuning_type_agent is None), every rate is 0 (:2231-2232) */
+  int64_t n_other;               /* 1 (every row sees row 0) or the number of rows */
+  int32_t n_pad;                 /* filled by riab_avc_pack */
+  int32_t reserved;
+} riab_avc_cells;
+/* Floats of the packed block: the riab_ovc_pack block without its type column, mu_d | s_d | cos(mu/2) | sin(mu/2) | k_q. */
+int64_t riab_avc_pack_floats(int32_t n_cells);
+/* tuning_angles / sigma_angles in radians (VectorCells attributes).  Fills n_cells and n_pad of meta_out. */
+int riab_avc_pack(const double* tuning_distances, const double* tuning_angles, const double* sigma_distances,
+                  const double* sigma_angles, int32_t n_cells, riab_avc_cells* meta_out, float* out_host);
+/* AgentVectorCells.get_state at given positions: other_pos_dev (n_pos,2) f64 when other_per_position, else one (2)
+ * partner position for every row (cells->other_pos_dev and partner_is_self are not read); head_direction_dev (n_pos,2)
+ * for egocentric cells, NULL = [1,0] (:2263-2278).  No noise, no NaN-position masking. */
+int riab_avc_rates(const double* pos_dev, int64_t n_pos, const double* other_pos_dev, int32_t other_per_position,
+                   const riab_env* env, const riab_avc_cells* cells, const double* head_direction_dev, float* out_dev,
+                   int64_t ld_out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
@@ -433,7 +465,7 @@ int riab_kin_rates(const double* vec_dev, int32_t vec_per_position, int64_t n_po
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
-                                   riab_rsn_cells* / riab_kin_cells* */
+                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

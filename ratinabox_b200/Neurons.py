@@ -781,6 +781,179 @@ class FieldOfViewOVCs(ObjectVectorCells):
         super().__init__(Agent, p)
 
 
+class AgentVectorCells(BoundaryVectorCells):
+    """ratinabox.AgentVectorCells (Neurons.py:2151-2320): vector cells tuned to another Agent, ``tuning_type_agent`` (the
+    ``Other_Agent`` argument).  A cell fires ``gaussian(d) * von_mises(bearing)`` of the vector from the agent to its
+    partner, with the other VectorCells' tuning machinery (cell_arrangement, tuning_distance, ...); ``walls_occlude`` takes
+    the line-of-sight distance (1000 behind an inner wall).
+
+    Pairing: row i of ``Agent`` sees row i of ``Other_Agent`` (``Other_Agent.n_agents == Agent.n_agents``, and under
+    sharding the same ``id_offset``), or every row sees the single agent of an ``Other_Agent`` with ``n_agents == 1``.
+    Passing the Agent itself pairs each agent with itself.  The partner's position is read as it stands when the rates are
+    evaluated: its queued motion step runs first, and its in-place edits are uploaded.  ``Agent.run`` does not move the
+    partner, like the reference's loop.  ``tuning_type_agent`` may be reassigned (another Agent, or None: zero rates).
+
+    Away from the agents (``evaluate_at="all"`` or ``pos=...``) the partner is ``Other_Agent.pos`` when it has one agent;
+    a batched partner needs the ``other_pos`` kwarg, one (2,) position or one per position.  Egocentric cells take the
+    ``head_direction`` kwarg there, like ObjectVectorCells.  Rates are evaluated by ``riab_avc_*`` (csrc/riab_avc.cuh)."""
+    default_params = {                                              # ratinabox/Neurons.py:2165-2168
+        "name": "AgentVectorCell",
+        "walls_occlude": True,          # agents behind walls cannot be seen
+    }
+    _cells_kind = _lib.CELLS_AVC
+    _egocentric_warning = ObjectVectorCells._egocentric_warning      # the reference's own text (Neurons.py:2274-2276)
+
+    def __init__(self, Agent, Other_Agent, params={}):
+        p = copy.deepcopy(__class__.default_params)
+        p.update(params)
+        Other_Agent.agent_idx                                        # the reference reads it for its colours (:2195)
+        warn_n = "n" in params and params["n"] is not None           # Neurons.py:2180-2181
+        Neurons.__init__(self, Agent, p)
+        self._init_vector_tuning()
+        if warn_n:                                                   # VectorCells.__init__, Neurons.py:1375-1379
+            arr = self.params["cell_arrangement"]
+            if (isinstance(arr, str) and arr.endswith("manifold")) or self.params["n"] != self.n:
+                warnings.warn(f"Ignoring 'n' parameter value ({self.params['n']}) that was passed, and setting number of "
+                              f"{self.name} neurons to {self.n}, inferred from the cell arrangement parameter.")
+        self.wall_geometry = "line_of_sight" if self.walls_occlude == True else "euclidean"      # Neurons.py:2188-2191
+        if Agent.Environment.boundary_conditions == "periodic":
+            raise NotImplementedError("AgentVectorCells need solid boundary conditions on the CUDA path")
+        self._check_partner(Other_Agent)
+        self.tuning_type_agent = Other_Agent
+
+    def _check_partner(self, other):
+        ag = self.Agent
+        if other is None or other is ag:
+            return
+        if other.n_agents not in (ag.n_agents, 1):
+            raise ValueError(f"Other_Agent has {other.n_agents} agents, this Agent {ag.n_agents}: AgentVectorCells pair row "
+                             "i with row i of Other_Agent, or every row with an Other_Agent of one agent")
+        if other.n_agents > 1 and int(other.id_offset) != int(ag.id_offset):
+            raise ValueError(f"Other_Agent's id_offset {other.id_offset} differs from this Agent's {ag.id_offset}: paired "
+                             "shards must cover the same global agent ids")
+        if other.device != ag.device:
+            raise ValueError(f"Other_Agent lives on {other.device}, this Agent on {ag.device}")
+
+    def _partner(self):
+        """The partner, with its queued motion step run and its in-place edits uploaded (the position the reference's
+        get_state would read now)."""
+        other = self.tuning_type_agent
+        if other is not None and other is not self.Agent:
+            other._flush_pending()
+            other._sync_user_writes()
+        return other
+
+    def _cells(self):
+        self._partner()
+        return super()._cells()
+
+    def _signature(self):
+        other = self.tuning_type_agent
+        return tuple(np.ascontiguousarray(a, dtype=np.float64).tobytes() for a in (
+            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)) + (
+            float(self.min_fr), float(self.max_fr), self.reference_frame, self.wall_geometry,
+            self.Agent.Environment._walls_signature(), id(other),
+            None if other is None else (other.n_agents, int(other.id_offset), other._s["pos"].data_ptr()))
+
+    def _pack(self):
+        other = self.tuning_type_agent
+        self._check_partner(other)
+        arrs = [np.ascontiguousarray(a, dtype=np.float64).reshape(-1) for a in (
+            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)]
+        self.n = arrs[0].shape[0]
+        c = _lib.AvcCells()
+        host = np.zeros(self._lib.riab_avc_pack_floats(self.n), dtype=np.float32)
+        _lib.check(self._lib.riab_avc_pack(*[_f64p(a) for a in arrs], self.n, C.byref(c), host.ctypes.data_as(_lib.c_float_p)))
+        self._packed = self._upload(host)
+        c.walls_occlude = 1 if self.wall_geometry == "line_of_sight" else 0
+        c.egocentric = 1 if self.reference_frame == "egocentric" else 0
+        c.partner_is_self = 1 if other is self.Agent else 0
+        c.min_fr, c.max_fr = float(self.min_fr), float(self.max_fr)
+        c.packed_dev = self._packed.data_ptr()
+        c.other_pos_dev = None if (other is None or other is self.Agent) else other._s["pos"].data_ptr()
+        c.n_other = 1 if (other is None or other is self.Agent) else other.n_agents
+        return c
+
+    def _scratch_ptr(self, n):
+        return None
+
+    def get_state(self, evaluate_at="agent", **kwargs):
+        """AgentVectorCells.get_state (Neurons.py:2204-2320): (n, n_pos) float64, or with ``return_tensor=True`` the
+        (n_pos, n) float32 device tensor.  Zeros without a partner (:2231-2232)."""
+        torch = self._torch
+        ag = self.Agent
+        cells = self._cells()
+        other = self.tuning_type_agent
+        ego = self.reference_frame == "egocentric"
+        hd_dev = None
+        if evaluate_at == "agent":
+            ag._flush_pending()
+            ag._sync_user_writes()
+            pos_dev = ag._s["pos"]
+            if ego:
+                hd_dev = ag._s["head_direction"]
+            other_dev = None if other is None else other._s["pos"]
+        else:
+            pos = ag.Environment.flattened_discrete_coords if evaluate_at == "all" else kwargs["pos"]
+            pos_dev = self._f64_rows(pos)
+            other_dev = None
+            if other is not None:
+                if "other_pos" in kwargs:
+                    other_dev = self._f64_rows(kwargs["other_pos"])
+                elif other.n_agents == 1:
+                    other_dev = other._s["pos"]
+                else:
+                    raise ValueError(f"Other_Agent has {other.n_agents} agents: pass their positions away from the agents "
+                                     "with other_pos=, one (2,) position or one per position")
+        n_pos = int(pos_dev.shape[0])
+        out = torch.zeros((n_pos, self._ld()), dtype=torch.float32, device=self.device)
+        if other_dev is not None and other_dev.shape[0] not in (1, n_pos):
+            raise ValueError(f"{other_dev.shape[0]} partner positions for {n_pos} positions: pass one (2,) position or one "
+                             "per position")
+        if other is not None and evaluate_at != "agent" and ego:
+            if "head_direction" in kwargs:
+                hd = np.array(kwargs["head_direction"], dtype=np.float64)
+            elif "vel" in kwargs:
+                warnings.warn("'vel' kwarg deprecated in favour of 'head_direction'")
+                hd = np.asarray(kwargs["vel"], dtype=np.float64)
+            else:
+                warnings.warn(self._egocentric_warning)
+                hd = np.array([1.0, 0.0])
+            hd_dev = torch.as_tensor(np.array(np.broadcast_to(hd.reshape(-1, 2), (n_pos, 2)), order="C"), device=self.device)
+        if other is not None and n_pos:
+            _lib.check(self._lib.riab_avc_rates(pos_dev.data_ptr(), n_pos, other_dev.data_ptr(),
+                                                1 if other_dev.shape[0] > 1 else 0, C.byref(ag._env_struct()),
+                                                C.byref(cells), None if hd_dev is None else hd_dev.data_ptr(),
+                                                out.data_ptr(), out.stride(0), ag._stream()))
+        if kwargs.get("return_tensor", False):
+            return out[:, : self.n]
+        return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
+
+    def _f64_rows(self, x):
+        torch = self._torch
+        if isinstance(x, torch.Tensor):
+            return x.to(device=self.device, dtype=torch.float64).reshape(-1, 2).contiguous()
+        return torch.as_tensor(np.ascontiguousarray(np.asarray(x, dtype=np.float64).reshape(-1, 2)), device=self.device)
+
+
+class FieldOfViewAVCs(AgentVectorCells):
+    """Egocentric AgentVectorCells tiling the agent's field of view (ratinabox/Neurons.py:2323-2351)."""
+    default_params = {
+        "distance_range": [0.02, 0.4],
+        "angle_range": [0, 75],
+        "spatial_resolution": 0.02,
+        "beta": 5,
+        "cell_arrangement": "diverging_manifold",
+    }
+
+    def __init__(self, Agent, Other_Agent, params={}):
+        p = copy.deepcopy(__class__.default_params)
+        p.update(params)
+        p["reference_frame"] = "egocentric"
+        assert p["cell_arrangement"] is not None, "cell_arrangement must be set for FOV Neurons"
+        super().__init__(Agent, Other_Agent, p)
+
+
 # =============================================================================
 class _FflInput(dict):
     """One entry of ``FeedForwardLayer.inputs`` with the reference's keys (Neurons.py:2781-2788).  ``"I"`` is looked up

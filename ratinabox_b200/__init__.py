@@ -12,8 +12,8 @@ from .Environment import Environment          # noqa: E402
 from .Agent import Agent                      # noqa: E402
 from .Neurons import (Neurons, PlaceCells, GridCells, BoundaryVectorCells, FieldOfViewBVCs,   # noqa: E402
                       ObjectVectorCells, FieldOfViewOVCs, FeedForwardLayer, RandomSpatialNeurons,
-                      HeadDirectionCells, VelocityCells, SpeedCell)
+                      HeadDirectionCells, VelocityCells, SpeedCell, AgentVectorCells, FieldOfViewAVCs)
 
 __all__ = ["Environment", "Agent", "Neurons", "PlaceCells", "GridCells", "BoundaryVectorCells", "FieldOfViewBVCs",
            "ObjectVectorCells", "FieldOfViewOVCs", "FeedForwardLayer", "RandomSpatialNeurons", "HeadDirectionCells",
-           "VelocityCells", "SpeedCell"]
+           "VelocityCells", "SpeedCell", "AgentVectorCells", "FieldOfViewAVCs"]

@@ -5,7 +5,7 @@
 //   k_agent_update_src  Agent.update from an imported trajectory / forced positions, one agent per thread (float64)
 //   k_traj_build        not-a-knot spline of imported trajectories, one thread per (trajectory, axis) column
 //   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells / ObjectVectorCells /
-//                       head direction, velocity and speed cells:
+//                       head direction, velocity and speed cells / AgentVectorCells:
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
@@ -24,6 +24,7 @@
 #include "riab_bvc.cuh"
 #include "riab_ffl.cuh"
 #include "riab_ovc.cuh"
+#include "riab_avc.cuh"
 #include "riab_grid.cuh"
 #include "riab_kin.cuh"
 #include "riab_motion.cuh"
@@ -367,7 +368,7 @@ struct PlacePolicy {
   static __device__ __forceinline__ void prepare(double* aux, const double* s_walls, const Const& c) {
     place_wall_invariants(aux, s_walls + 4 * c.wall0, WI > 0 ? c.n_inner : 0);
   }
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, double, double, double, double,
+  static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double, double, double, double, double, double,
                                                 const double* s_walls, const double* aux, const Const& c, const EnvK& env) {
     place_agent_record<WI>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
   }
@@ -391,7 +392,7 @@ struct GridPolicy {
   static constexpr bool POSITIONAL = true;
   static __device__ __forceinline__ void given_dir(const Const&, long long, double&, double&) {}
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double, double, double, double, double, double,
+  static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double, double, double, double, double, double,
                                                 const double*, const double*, const Const&, const EnvK& env) {
     rec[0] = (float)(px - env.cxm);
     rec[1] = (float)(py - env.cym);
@@ -418,7 +419,7 @@ struct OvcPolicy {
     if (c.head_dir != nullptr) { x = c.head_dir[2 * i]; y = c.head_dir[2 * i + 1]; }
   }
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
-  static __device__ __forceinline__ void record(float* rec, double px, double py, double hdx, double hdy, double, double,
+  static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double hdx, double hdy, double, double,
                                                 double, double, const double* s_walls, const double*, const Const& c,
                                                 const EnvK&) {
     ovc_agent_record(rec, px, py, hdx, hdy, s_walls, c);
@@ -446,7 +447,7 @@ struct KinPolicy {
     if (c.vec != nullptr) { x = c.vec[c.vec_ld * i]; y = c.vec[c.vec_ld * i + 1]; }
   }
   static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
-  static __device__ __forceinline__ void record(float* rec, double, double, double hdx, double hdy, double vx, double vy,
+  static __device__ __forceinline__ void record(float* rec, long long, double, double, double hdx, double hdy, double vx, double vy,
                                                 double mvx, double mvy, const double*, const double*, const Const& c,
                                                 const EnvK&) {
     kin_agent_record(rec, hdx, hdy, vx, vy, mvx, mvy, c);
@@ -456,6 +457,35 @@ struct KinPolicy {
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
                                                 uint32_t, bool&) {
     kin_rates4(o, r, c, rec);
+  }
+  static __device__ __forceinline__ int expanded(const Const&) { return 0; }
+  static __device__ __forceinline__ int wall0(const Const&) { return 0; }
+};
+
+// AgentVectorCells: OvcPolicy's geometry for one "object", the partner Agent's position of the record's row.
+struct AvcPolicy {
+  using Const = AvcConst;
+  using Regs = AvcCellRegs;
+  static constexpr int REC = AVC_REC;
+  // 20 cell registers: as a LIGHT policy, ptxas -v reports 56-60 spill bytes in its StepCfg<8> instantiations (KinPolicy's
+  // 12 registers: 28-32), so the consumers keep the 96-register configurations like OvcPolicy
+  static constexpr bool LIGHT = false;
+  static constexpr bool THIN = false;     // the dense spike stream, as for OVC (a NaN partner gives NaN rates)
+  static constexpr bool POSITIONAL = true;
+  static __device__ __forceinline__ void given_dir(const Const& c, long long i, double& x, double& y) {
+    if (c.head_dir != nullptr) { x = c.head_dir[2 * i]; y = c.head_dir[2 * i + 1]; }
+  }
+  static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
+  static __device__ __forceinline__ void record(float* rec, long long i, double px, double py, double hdx, double hdy, double,
+                                                double, double, double, const double* s_walls, const double*, const Const& c,
+                                                const EnvK&) {
+    avc_agent_record(rec, px, py, hdx, hdy, i, s_walls, c);
+  }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { avc_load_cells(r, c, cell0); }
+  template <bool DEFER, int EXP = -1>
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
+                                                uint32_t, bool&) {
+    avc_rates4(o, r, c, rec);
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const&) { return 0; }
@@ -961,7 +991,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             if constexpr (MODE == 4) agent_update_src_one(ag, mp, md, io_st, run.src, t_st, env, a0 + lane, as);
             else agent_update_one<false>(ag, mp, md, io_st, env, s_walls, a0 + lane, as);
             nanpos = (as.px != as.px);
-            P::record(s_slot[s].rec[lane], as.px, as.py, as.hdx, as.hdy, as.vx, as.vy, as.mvx, as.mvy, s_walls, s_aux, pc, env);
+            P::record(s_slot[s].rec[lane], a0 + lane, as.px, as.py, as.hdx, as.hdy, as.vx, as.vy, as.mvx, as.mvy, s_walls, s_aux, pc, env);
           }
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
         }
@@ -984,7 +1014,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             const long long i = a0 + lane;
             const double px = ag.pos[2 * i], py = ag.pos[2 * i + 1];
             nanpos = (px != px);
-            P::record(s_slot[s].rec[lane], px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], ag.velocity[2 * i],
+            P::record(s_slot[s].rec[lane], i, px, py, ag.head_direction[2 * i], ag.head_direction[2 * i + 1], ag.velocity[2 * i],
                       ag.velocity[2 * i + 1], ag.measured_velocity[2 * i], ag.measured_velocity[2 * i + 1], s_walls, s_aux, pc, env);
           }
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
@@ -1008,7 +1038,7 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
             vx = mvx = hdx; vy = mvy = hdy;
           }
           nanpos = (px != px);
-          P::record(s_slot[s].rec[lane], px, py, hdx, hdy, vx, vy, mvx, mvy, s_walls, s_aux, pc, env);
+          P::record(s_slot[s].rec[lane], i, px, py, hdx, hdy, vx, vy, mvx, mvy, s_walls, s_aux, pc, env);
         }
         publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
       }
@@ -1675,6 +1705,30 @@ int make_kin(const riab_kin_cells* kc, const riab_agents& ag, KinConst& c) {
   return 0;
 }
 
+// AgentVectorCells over n_rows rows (the agents, or get_state's positions): the partner of each row (riab_avc_cells).
+int make_avc(const riab_avc_cells* vc, const EnvK& env, const double* head_dir, long long n_rows, AvcConst& c) {
+  if (vc == nullptr || vc->packed_dev == nullptr) return fail(RIAB_ERR_INVALID, "agent vector cells / packed_dev NULL");
+  if (vc->n_cells <= 0 || vc->n_pad != (vc->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD)
+    return fail(RIAB_ERR_INVALID, "agent vector cells: n_cells %d / n_pad %d (pack with riab_avc_pack)", vc->n_cells, vc->n_pad);
+  if (((uintptr_t)vc->packed_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "agent vector cells: packed_dev must be 16-byte aligned");
+  if (env.periodic) return fail(RIAB_ERR_UNSUPPORTED, "agent vector cells need solid boundary conditions here");
+  const bool partner = vc->partner_is_self == 0 && vc->other_pos_dev != nullptr;
+  if (partner && vc->n_other != 1 && vc->n_other != n_rows)
+    return fail(RIAB_ERR_INVALID, "agent vector cells: %lld partner rows for %lld rows (pair row by row, or one partner)",
+                (long long)vc->n_other, n_rows);
+  memset(&c, 0, sizeof(c));
+  c.n_cells = vc->n_cells; c.n_pad = vc->n_pad;
+  c.ego = vc->egocentric ? 1 : 0; c.occlude = vc->walls_occlude ? 1 : 0; c.self = vc->partner_is_self ? 1 : 0;
+  c.wall0 = env.W < 4 ? env.W : 4;                       // Environment.py:715-717: walls[4:]
+  c.n_inner = env.W - c.wall0;
+  const bool none = !c.self && vc->other_pos_dev == nullptr;
+  c.min_fr = none ? 0.f : vc->min_fr; c.span = none ? 0.f : vc->max_fr - vc->min_fr;   // no partner: zeros (Neurons.py:2231)
+  c.packed = vc->packed_dev; c.head_dir = head_dir;
+  c.other = c.self ? nullptr : vc->other_pos_dev;
+  c.other_ld = (vc->n_other == 1) ? 0 : 2;
+  return 0;
+}
+
 int g_num_sms = 0;
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
@@ -2078,7 +2132,7 @@ struct Pop {
   int kind = -1, n_cells = 0;
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
-  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin;
+  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
   const riab_rsn_cells* rsn = nullptr;  // its sample points: `place`
@@ -2115,6 +2169,9 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   } else if (kind == RIAB_CELLS_KIN) {
     rc = make_kin((const riab_kin_cells*)cells, ag, d.kin);
     d.n_cells = d.kin.n_cells;
+  } else if (kind == RIAB_CELLS_AVC) {
+    rc = make_avc((const riab_avc_cells*)cells, ek, ag.head_direction, ag.n_agents, d.avc);
+    d.n_cells = d.avc.n_cells;
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
@@ -2134,6 +2191,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
   if (d.kind == RIAB_CELLS_GRID) return launch_tile<GridPolicy, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, ag.n_agents, s);
   if constexpr (MODE == 0) {
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
@@ -2307,7 +2365,7 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
   const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
                        ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
-  // Skewed schedule (population 0 is a Place / Grid / OVC / kinematic population): motion(0) alone, then per step one kernel that
+  // Skewed schedule (population 0 is a Place / Grid / OVC / kinematic / AVC population): motion(0) alone, then per step one kernel that
   // evaluates rates(s) of the current positions while its producer warps already run motion(s+1); the last step is rates
   // only.  Same results as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source
   // keeps the plain schedule (its motion kernel is cheap next to the rates).
@@ -2812,6 +2870,40 @@ int riab_kin_rates(const double* vec_dev, int32_t vec_per_position, int64_t n_po
   d.kin.vec_ld = vec_per_position ? 2 : 0;
   d.kin.fixed_scale = speed_scale;
   return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------ AgentVectorCells
+int64_t riab_avc_pack_floats(int32_t n_cells) { return (int64_t)place_n_pad(n_cells) * 5; }
+
+int riab_avc_pack(const double* tuning_distances, const double* tuning_angles, const double* sigma_distances,
+                  const double* sigma_angles, int32_t n, riab_avc_cells* meta, float* out) {
+  if (!tuning_distances || !tuning_angles || !sigma_distances || !sigma_angles || !meta || !out || n <= 0)
+    return fail(RIAB_ERR_INVALID, "riab_avc_pack: bad argument");
+  const int np = place_n_pad(n);
+  const double log2e = 1.4426950408889634;
+  for (int i = 0; i < np; ++i) {                       // riab_ovc_pack's first five columns; pads (0, 0, 1, 0, 0)
+    const bool in = i < n;
+    const double kappa = in ? 1.0 / (sigma_angles[i] * sigma_angles[i]) : 0.0;       // utils.von_mises (utils.py:441-457)
+    out[i] = in ? (float)tuning_distances[i] : 0.f;
+    out[(size_t)np + i] = in ? (float)(sqrt(0.5 * log2e) / sigma_distances[i]) : 0.f;  // utils.gaussian (utils.py:424-438)
+    out[(size_t)2 * np + i] = in ? (float)cos(0.5 * tuning_angles[i]) : 1.f;
+    out[(size_t)3 * np + i] = in ? (float)sin(0.5 * tuning_angles[i]) : 0.f;
+    out[(size_t)4 * np + i] = (float)sqrt(2.0 * kappa * log2e);
+  }
+  meta->n_cells = n;
+  meta->n_pad = np;
+  return 0;
+}
+
+int riab_avc_rates(const double* pos_dev, int64_t n_pos, const double* other_pos_dev, int32_t other_per_position,
+                   const riab_env* env, const riab_avc_cells* cells, const double* head_direction_dev, float* out_dev,
+                   int64_t ld_out, void* stream) {
+  if (cells == nullptr || other_pos_dev == nullptr) return fail(RIAB_ERR_INVALID, "riab_avc_rates: bad argument");
+  riab_avc_cells c = *cells;
+  c.other_pos_dev = other_pos_dev;
+  c.n_other = other_per_position ? n_pos : 1;
+  c.partner_is_self = 0;
+  return rates_at(RIAB_CELLS_AVC, &c, pos_dev, n_pos, env, head_direction_dev, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ------------------------------------------------------------ ObjectVectorCells
