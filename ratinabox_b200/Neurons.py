@@ -1,6 +1,7 @@
-"""Host mirror of ``ratinabox.Neurons`` for PlaceCells, GridCells and allocentric
-BoundaryVectorCells: ``update()`` and ``get_state()`` run on the GPU through
-libriab_b200 (C ABI: include/riab_b200.h).
+"""Host mirror of ``ratinabox.Neurons``: PlaceCells, GridCells, the VectorCells (Boundary-, Object- and AgentVectorCells,
+allocentric or egocentric, and their FieldOfView forms), RandomSpatialNeurons, HeadDirectionCells, VelocityCells,
+SpeedCell and FeedForwardLayer.  ``update()`` and ``get_state()`` run on the GPU through libriab_b200 (C ABI:
+include/riab_b200.h).
 
 API parity (ratinabox/Neurons.py): ``Neurons(Agent, params)`` registers itself in
 ``Agent.Neurons`` (:111-112); ``update(**kwargs)`` (:145-171) refreshes
@@ -109,9 +110,8 @@ class Neurons:
     def _ld(self):
         return (self.n + 3) // 4 * 4
 
-    def _upload(self, host, dtype=None):
-        t = self._torch.as_tensor(np.ascontiguousarray(host), device=self.device)
-        return t
+    def _upload(self, host):
+        return self._torch.as_tensor(np.ascontiguousarray(host), device=self.device)
 
     def _row_buffers(self):
         """Next history row (rates [+ spikes]) on the device; grows / wraps like Agent's ring."""
@@ -233,26 +233,66 @@ class Neurons:
         return None
 
     # ----------------------------------------------------------------- get_state
+    _zeroed_state = False         # get_state's rates start as zeros (for populations whose kernel may not run)
+
     def get_state(self, evaluate_at="agent", **kwargs):
         """(n_cells, n_pos) firing rates, float64 NumPy (pass ``return_tensor=True``
         for the (n_pos, n_cells) float32 device tensor)."""
         torch = self._torch
         self._cells()
-        if evaluate_at == "agent":
-            self.Agent._flush_pending()
-            self.Agent._sync_user_writes()
-            pos_dev = self.Agent._s["pos"]
-        else:
-            pos = self.Agent.Environment.flattened_discrete_coords if evaluate_at == "all" else kwargs["pos"]
-            if isinstance(pos, torch.Tensor):
-                pos_dev = pos.to(device=self.device, dtype=torch.float64).reshape(-1, 2).contiguous()
-            else:
-                pos_dev = torch.as_tensor(np.ascontiguousarray(np.asarray(pos, dtype=np.float64).reshape(-1, 2)),
-                                          device=self.device)
+        pos_dev = self._positions(evaluate_at, kwargs)
         n_pos = int(pos_dev.shape[0])
-        out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
-        self._rates_from_positions(pos_dev, n_pos, out)
-        if kwargs.get("return_tensor", False):
+        inputs = self._kernel_inputs(evaluate_at, n_pos, kwargs)
+        out = (torch.zeros if self._zeroed_state else torch.empty)((n_pos, self._ld()), dtype=torch.float32,
+                                                                   device=self.device)
+        if n_pos:
+            self._rates_from_positions(pos_dev, n_pos, out, **inputs)
+        return self._result(out, kwargs.get("return_tensor", False))
+
+    def _agent_state(self):
+        """The Agent's device state as it stands now: its queued motion step run, the user's in-place edits of its
+        arrays (``Ag.pos``, ``Ag.head_direction`` ...) uploaded."""
+        self.Agent._flush_pending()
+        self.Agent._sync_user_writes()
+        return self.Agent._s
+
+    def _positions(self, evaluate_at, kwargs):
+        """get_state's points as a (n_pos, 2) float64 device tensor: the agents' positions at "agent", the discretised
+        environment at "all", else the ``pos`` kwarg."""
+        if evaluate_at == "agent":
+            return self._agent_state()["pos"]
+        return self._rows(self.Agent.Environment.flattened_discrete_coords if evaluate_at == "all" else kwargs["pos"])
+
+    def _n_pos(self, evaluate_at, kwargs, default):
+        """How many points get_state evaluates away from the agents, for populations that need only the count: the
+        discretised environment's for "all", the ``pos`` kwarg's rows, else ``default``."""
+        if evaluate_at == "all":
+            return self.Agent.Environment.flattened_discrete_coords.shape[0]
+        if "pos" in kwargs:
+            pos = kwargs["pos"]
+            return int((pos if isinstance(pos, self._torch.Tensor) else np.asarray(pos)).reshape(-1, 2).shape[0])
+        return default
+
+    def _rows(self, x, n=None):
+        """``x`` (NumPy, a list, or a torch tensor on any device) as a C-contiguous (k, 2) float64 device tensor; with
+        ``n``, broadcast to (n, 2)."""
+        torch = self._torch
+        if isinstance(x, torch.Tensor):
+            x = x.to(device=self.device, dtype=torch.float64).reshape(-1, 2)
+            return (x if n is None else x.expand(n, 2)).contiguous()
+        x = np.asarray(x, dtype=np.float64).reshape(-1, 2)
+        if n is not None:
+            x = np.array(np.broadcast_to(x, (n, 2)), order="C")          # own, writable copy
+        return torch.as_tensor(np.ascontiguousarray(x), device=self.device)
+
+    def _kernel_inputs(self, evaluate_at, n_pos, kwargs):
+        """Keyword arguments of ``_rates_from_positions`` besides the positions (head directions, partner positions)."""
+        return {}
+
+    def _result(self, out, return_tensor):
+        """get_state's value from its (n_pos, ld) float32 rates: the (n_pos, n) device view with ``return_tensor``, else
+        the (n, n_pos) float64 NumPy array."""
+        if return_tensor:
             return out[:, : self.n]
         return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
 
@@ -512,10 +552,12 @@ class GridCells(Neurons):
 
 
 # =============================================================================
-class BoundaryVectorCells(Neurons):
-    default_params = {                                              # Neurons.py:1303-1316 (VectorCells) + :1549-1555
+class VectorCells(Neurons):
+    """ratinabox.VectorCells (Neurons.py:1259-1437), the parent of BoundaryVectorCells, ObjectVectorCells and
+    AgentVectorCells: their shared tuning (``tuning_distances``, ``tuning_angles``, ``sigma_distances``, ``sigma_angles``
+    from ``cell_arrangement``) and the head directions egocentric cells read in get_state."""
+    default_params = {                                              # ratinabox/Neurons.py:1303-1316
         "n": 10,
-        "name": "BoundaryVectorCells",
         "reference_frame": "allocentric",
         "cell_arrangement": "random",
         "tuning_distance_distribution": "uniform",
@@ -526,12 +568,7 @@ class BoundaryVectorCells(Neurons):
         "tuning_angle": (0.0, 360),
         "angular_spread_distribution": "uniform",
         "angular_spread": (10, 30),
-        "dtheta": 2,
-        "max_fr": 1.0,
-        "min_fr": 0.0,
     }
-    _cells_kind = _lib.CELLS_BVC
-    _egocentric_warning = "BVCs in egocentric plane require a head direction vector but none was passed. Using [1,0]"
 
     def _init_vector_tuning(self):
         """VectorCells.set_tuning_parameters (Neurons.py:1388-1437): tuning_distances / tuning_angles /
@@ -557,6 +594,44 @@ class BoundaryVectorCells(Neurons):
             "All manifold tuning parameters must be of the same length"
         self.n = len(self.tuning_distances)
 
+    def _vector_tuning(self):
+        """The four tuning arrays as contiguous float64 vectors, in the packers' order."""
+        return [np.ascontiguousarray(a, dtype=np.float64).reshape(-1) for a in (
+            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)]
+
+    def _kernel_inputs(self, evaluate_at, n_pos, kwargs):
+        if self.reference_frame != "egocentric":
+            return {}
+        return {"head_dir": self._head_directions(evaluate_at, n_pos, kwargs)}
+
+    def _head_directions(self, evaluate_at, n_pos, kwargs):
+        """The (n_pos, 2) float64 device head directions of egocentric cells: the agents' at "agent", else the
+        ``head_direction`` kwarg (one vector for all positions, or one per position), the deprecated ``vel``, or [1,0]
+        with the reference's warning (Neurons.py:1693-1706)."""
+        if evaluate_at == "agent":
+            return self._agent_state()["head_direction"]
+        if "head_direction" in kwargs:
+            hd = kwargs["head_direction"]
+        elif "vel" in kwargs:
+            warnings.warn("'vel' kwarg deprecated in favour of 'head_direction'")
+            hd = kwargs["vel"]
+        else:
+            warnings.warn(self._egocentric_warning)
+            hd = [1.0, 0.0]
+        return self._rows(hd, n_pos)
+
+
+class BoundaryVectorCells(VectorCells):
+    default_params = {                                              # ratinabox/Neurons.py:1549-1555
+        "n": 10,
+        "name": "BoundaryVectorCells",
+        "dtheta": 2,
+        "max_fr": 1.0,
+        "min_fr": 0.0,
+    }
+    _cells_kind = _lib.CELLS_BVC
+    _egocentric_warning = "BVCs in egocentric plane require a head direction vector but none was passed. Using [1,0]"
+
     def __init__(self, Agent, params={}):
         from .utils import rotate
         super().__init__(Agent, params)
@@ -577,12 +652,11 @@ class BoundaryVectorCells(Neurons):
 
     def _signature(self):
         return tuple(np.ascontiguousarray(a, dtype=np.float64).tobytes() for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles, self.test_angles,
-            self.test_directions)) + (float(self.min_fr), float(self.max_fr), self.reference_frame)
+            *self._vector_tuning(), self.test_angles, self.test_directions)) + (
+            float(self.min_fr), float(self.max_fr), self.reference_frame)
 
     def _pack(self):
-        arrs = [np.ascontiguousarray(a, dtype=np.float64).reshape(-1) for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)]
+        arrs = self._vector_tuning()
         self.n = arrs[0].shape[0]
         angs = np.ascontiguousarray(self.test_angles, dtype=np.float64)
         T = angs.shape[0]
@@ -616,38 +690,6 @@ class BoundaryVectorCells(Neurons):
                                             head_dir.data_ptr() if head_dir is not None else None,
                                             out.data_ptr(), out.stride(0), ag._stream()))
 
-    def get_state(self, evaluate_at="agent", **kwargs):
-        """BoundaryVectorCells.get_state (Neurons.py:1617-1744).  Egocentric cells take the Agent's
-        head_direction with evaluate_at="agent", else the ``head_direction`` kwarg (one vector for all
-        positions, or one per position), else [1,0] with the reference's warning (Neurons.py:1693-1706)."""
-        if self.reference_frame != "egocentric":
-            return super().get_state(evaluate_at, **kwargs)
-        torch = self._torch
-        self._cells()
-        if evaluate_at == "agent":
-            self.Agent._flush_pending()
-            pos_dev, hd_dev = self.Agent._s["pos"], self.Agent._s["head_direction"]
-        else:
-            pos = self.Agent.Environment.flattened_discrete_coords if evaluate_at == "all" else kwargs["pos"]
-            pos_dev = torch.as_tensor(np.ascontiguousarray(np.asarray(pos, dtype=np.float64).reshape(-1, 2)), device=self.device)
-            if "head_direction" in kwargs:
-                hd = np.array(kwargs["head_direction"], dtype=np.float64)       # own, writable copy
-            elif "vel" in kwargs:
-                warnings.warn("'vel' kwarg deprecated in favour of 'head_direction'")
-                hd = np.asarray(kwargs["vel"], dtype=np.float64)
-            else:
-                warnings.warn(self._egocentric_warning)
-                hd = np.array([1.0, 0.0])
-            hd = np.array(np.broadcast_to(hd.reshape(-1, 2), (pos_dev.shape[0], 2)), order="C")   # own, writable, C-contiguous
-            hd_dev = torch.as_tensor(hd, device=self.device)
-        n_pos = int(pos_dev.shape[0])
-        out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
-        if n_pos:
-            self._rates_from_positions(pos_dev, n_pos, out, head_dir=hd_dev)
-        if kwargs.get("return_tensor", False):
-            return out[:, : self.n]
-        return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
-
 
 class FieldOfViewBVCs(BoundaryVectorCells):
     """Egocentric BVCs tiling the agent's field of view (ratinabox/Neurons.py:1847-1887)."""
@@ -668,7 +710,7 @@ class FieldOfViewBVCs(BoundaryVectorCells):
         super().__init__(Agent, p)
 
 
-class ObjectVectorCells(BoundaryVectorCells):
+class ObjectVectorCells(VectorCells):
     """ratinabox.ObjectVectorCells (Neurons.py:1892-2113): vector cells tuned to the objects of the Environment.
     Same tuning machinery as the other VectorCells (cell_arrangement, tuning_distance, ...); each cell responds to the
     objects of ONE type (``object_tuning_type``: "random", an int, or one int per cell).  The rates are evaluated by
@@ -689,7 +731,7 @@ class ObjectVectorCells(BoundaryVectorCells):
             raise RuntimeError(f"Cannot initialize {p['name']}, as there are no objects in the environment.")
         if len(env.objects["objects"]) > _lib.MAX_OBJECTS:
             raise NotImplementedError(f"at most {_lib.MAX_OBJECTS} objects per environment on the CUDA path")
-        Neurons.__init__(self, Agent, p)
+        super().__init__(Agent, p)
         self._init_vector_tuning()
         self.object_locations = env.objects["objects"]
         self.tuning_types = None
@@ -713,15 +755,13 @@ class ObjectVectorCells(BoundaryVectorCells):
     def _signature(self):
         env = self.Agent.Environment
         return tuple(np.ascontiguousarray(a, dtype=np.float64).tobytes() for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles,
-            np.asarray(self.tuning_types, dtype=np.float64), env.objects["objects"],
+            *self._vector_tuning(), np.asarray(self.tuning_types, dtype=np.float64), env.objects["objects"],
             np.asarray(env.objects["object_types"], dtype=np.float64))) + (
             float(self.min_fr), float(self.max_fr), self.reference_frame, self.wall_geometry)
 
     def _pack(self):
         env = self.Agent.Environment
-        arrs = [np.ascontiguousarray(a, dtype=np.float64).reshape(-1) for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)]
+        arrs = self._vector_tuning()
         self.n = arrs[0].shape[0]
         types = np.ascontiguousarray(self.tuning_types, dtype=np.int32).reshape(-1)
         assert types.shape[0] == self.n
@@ -744,10 +784,7 @@ class ObjectVectorCells(BoundaryVectorCells):
         c.packed_dev = self._packed.data_ptr()
         return c
 
-    def _scratch_ptr(self, n):
-        return None
-
-    def _rates_from_positions(self, pos_dev, n_pos, out, first_wall=None, head_dir=None):
+    def _rates_from_positions(self, pos_dev, n_pos, out, head_dir=None):
         ag = self.Agent
         _lib.check(self._lib.riab_ovc_rates(pos_dev.data_ptr(), n_pos, C.byref(ag._env_struct()), C.byref(self._cells()),
                                             head_dir.data_ptr() if head_dir is not None else None,
@@ -781,7 +818,7 @@ class FieldOfViewOVCs(ObjectVectorCells):
         super().__init__(Agent, p)
 
 
-class AgentVectorCells(BoundaryVectorCells):
+class AgentVectorCells(VectorCells):
     """ratinabox.AgentVectorCells (Neurons.py:2151-2320): vector cells tuned to another Agent, ``tuning_type_agent`` (the
     ``Other_Agent`` argument).  A cell fires ``gaussian(d) * von_mises(bearing)`` of the vector from the agent to its
     partner, with the other VectorCells' tuning machinery (cell_arrangement, tuning_distance, ...); ``walls_occlude`` takes
@@ -802,13 +839,14 @@ class AgentVectorCells(BoundaryVectorCells):
     }
     _cells_kind = _lib.CELLS_AVC
     _egocentric_warning = ObjectVectorCells._egocentric_warning      # the reference's own text (Neurons.py:2274-2276)
+    _zeroed_state = True                                             # zeros without a partner (:2231-2232)
 
     def __init__(self, Agent, Other_Agent, params={}):
         p = copy.deepcopy(__class__.default_params)
         p.update(params)
         Other_Agent.agent_idx                                        # the reference reads it for its colours (:2195)
         warn_n = "n" in params and params["n"] is not None           # Neurons.py:2180-2181
-        Neurons.__init__(self, Agent, p)
+        super().__init__(Agent, p)
         self._init_vector_tuning()
         if warn_n:                                                   # VectorCells.__init__, Neurons.py:1375-1379
             arr = self.params["cell_arrangement"]
@@ -849,8 +887,7 @@ class AgentVectorCells(BoundaryVectorCells):
 
     def _signature(self):
         other = self.tuning_type_agent
-        return tuple(np.ascontiguousarray(a, dtype=np.float64).tobytes() for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)) + (
+        return tuple(a.tobytes() for a in self._vector_tuning()) + (
             float(self.min_fr), float(self.max_fr), self.reference_frame, self.wall_geometry,
             self.Agent.Environment._walls_signature(), id(other),
             None if other is None else (other.n_agents, int(other.id_offset), other._s["pos"].data_ptr()))
@@ -858,8 +895,7 @@ class AgentVectorCells(BoundaryVectorCells):
     def _pack(self):
         other = self.tuning_type_agent
         self._check_partner(other)
-        arrs = [np.ascontiguousarray(a, dtype=np.float64).reshape(-1) for a in (
-            self.tuning_distances, self.tuning_angles, self.sigma_distances, self.sigma_angles)]
+        arrs = self._vector_tuning()
         self.n = arrs[0].shape[0]
         c = _lib.AvcCells()
         host = np.zeros(self._lib.riab_avc_pack_floats(self.n), dtype=np.float32)
@@ -874,66 +910,34 @@ class AgentVectorCells(BoundaryVectorCells):
         c.n_other = 1 if (other is None or other is self.Agent) else other.n_agents
         return c
 
-    def _scratch_ptr(self, n):
-        return None
-
-    def get_state(self, evaluate_at="agent", **kwargs):
-        """AgentVectorCells.get_state (Neurons.py:2204-2320): (n, n_pos) float64, or with ``return_tensor=True`` the
-        (n_pos, n) float32 device tensor.  Zeros without a partner (:2231-2232)."""
-        torch = self._torch
-        ag = self.Agent
-        cells = self._cells()
+    def _kernel_inputs(self, evaluate_at, n_pos, kwargs):
+        """The partner's positions (its agents' at "agent", else the ``other_pos`` kwarg or a one-agent partner's
+        position) and, for egocentric cells, the head directions; nothing without a partner."""
         other = self.tuning_type_agent
-        ego = self.reference_frame == "egocentric"
-        hd_dev = None
+        if other is None:
+            return {}
         if evaluate_at == "agent":
-            ag._flush_pending()
-            ag._sync_user_writes()
-            pos_dev = ag._s["pos"]
-            if ego:
-                hd_dev = ag._s["head_direction"]
-            other_dev = None if other is None else other._s["pos"]
+            other_pos = other._s["pos"]
+        elif "other_pos" in kwargs:
+            other_pos = self._rows(kwargs["other_pos"])
+        elif other.n_agents == 1:
+            other_pos = other._s["pos"]
         else:
-            pos = ag.Environment.flattened_discrete_coords if evaluate_at == "all" else kwargs["pos"]
-            pos_dev = self._f64_rows(pos)
-            other_dev = None
-            if other is not None:
-                if "other_pos" in kwargs:
-                    other_dev = self._f64_rows(kwargs["other_pos"])
-                elif other.n_agents == 1:
-                    other_dev = other._s["pos"]
-                else:
-                    raise ValueError(f"Other_Agent has {other.n_agents} agents: pass their positions away from the agents "
-                                     "with other_pos=, one (2,) position or one per position")
-        n_pos = int(pos_dev.shape[0])
-        out = torch.zeros((n_pos, self._ld()), dtype=torch.float32, device=self.device)
-        if other_dev is not None and other_dev.shape[0] not in (1, n_pos):
-            raise ValueError(f"{other_dev.shape[0]} partner positions for {n_pos} positions: pass one (2,) position or one "
+            raise ValueError(f"Other_Agent has {other.n_agents} agents: pass their positions away from the agents "
+                             "with other_pos=, one (2,) position or one per position")
+        if other_pos.shape[0] not in (1, n_pos):
+            raise ValueError(f"{other_pos.shape[0]} partner positions for {n_pos} positions: pass one (2,) position or one "
                              "per position")
-        if other is not None and evaluate_at != "agent" and ego:
-            if "head_direction" in kwargs:
-                hd = np.array(kwargs["head_direction"], dtype=np.float64)
-            elif "vel" in kwargs:
-                warnings.warn("'vel' kwarg deprecated in favour of 'head_direction'")
-                hd = np.asarray(kwargs["vel"], dtype=np.float64)
-            else:
-                warnings.warn(self._egocentric_warning)
-                hd = np.array([1.0, 0.0])
-            hd_dev = torch.as_tensor(np.array(np.broadcast_to(hd.reshape(-1, 2), (n_pos, 2)), order="C"), device=self.device)
-        if other is not None and n_pos:
-            _lib.check(self._lib.riab_avc_rates(pos_dev.data_ptr(), n_pos, other_dev.data_ptr(),
-                                                1 if other_dev.shape[0] > 1 else 0, C.byref(ag._env_struct()),
-                                                C.byref(cells), None if hd_dev is None else hd_dev.data_ptr(),
-                                                out.data_ptr(), out.stride(0), ag._stream()))
-        if kwargs.get("return_tensor", False):
-            return out[:, : self.n]
-        return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
+        return dict(super()._kernel_inputs(evaluate_at, n_pos, kwargs), other_pos=other_pos)
 
-    def _f64_rows(self, x):
-        torch = self._torch
-        if isinstance(x, torch.Tensor):
-            return x.to(device=self.device, dtype=torch.float64).reshape(-1, 2).contiguous()
-        return torch.as_tensor(np.ascontiguousarray(np.asarray(x, dtype=np.float64).reshape(-1, 2)), device=self.device)
+    def _rates_from_positions(self, pos_dev, n_pos, out, head_dir=None, other_pos=None):
+        if other_pos is None:
+            return                                                   # no partner: the zeros get_state allocated
+        ag = self.Agent
+        _lib.check(self._lib.riab_avc_rates(pos_dev.data_ptr(), n_pos, other_pos.data_ptr(),
+                                            1 if other_pos.shape[0] > 1 else 0, C.byref(ag._env_struct()),
+                                            C.byref(self._cells()), None if head_dir is None else head_dir.data_ptr(),
+                                            out.data_ptr(), out.stride(0), ag._stream()))
 
 
 class FieldOfViewAVCs(AgentVectorCells):
@@ -1135,13 +1139,7 @@ class FeedForwardLayer(Neurons):
             fc = _lib.FflCells.from_buffer_copy(c)
             fc.prime_dev = None
             keep = []
-            if evaluate_at == "all":
-                n_pos = self.Agent.Environment.flattened_discrete_coords.shape[0]
-            elif "pos" in kwargs:
-                n_pos = int(np.asarray(kwargs["pos"]).reshape(-1, 2).shape[0]) if not isinstance(kwargs["pos"], torch.Tensor) \
-                    else int(kwargs["pos"].reshape(-1, 2).shape[0])
-            else:
-                n_pos = self.Agent.n_agents
+            n_pos = self._n_pos(evaluate_at, kwargs, self.Agent.n_agents)
             for i, e in enumerate(self.inputs.values()):
                 pass_max = max_recurrence
                 if max_recurrence is not None and e["recurrent"]:
@@ -1162,10 +1160,8 @@ class FeedForwardLayer(Neurons):
         ro = _lib.RatesOut()
         ro.rates_row, ro.ld = out.data_ptr(), self._ld()
         _lib.check(self._lib.riab_ffl_rates(C.byref(fc), n_pos, None, None, C.byref(ro), self.Agent._stream()))
-        if return_tensor:
-            return out[:, : self.n]
-        r = out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
-        return r[:, 0] if (evaluate_at == "last" and n_pos == 1) else r
+        r = self._result(out, return_tensor)
+        return r[:, 0] if (evaluate_at == "last" and n_pos == 1 and not return_tensor) else r
 
 
 # =============================================================================
@@ -1307,23 +1303,12 @@ class _KinematicCells(Neurons):
         c = _lib.KinCells.from_buffer_copy(self._cells())
         c.use_velocity = 1 if use_velocity else 0
         if evaluate_at == "agent":
-            ag._flush_pending()
-            ag._sync_user_writes()
-            vec = ag._s["measured_velocity" if self._variant == _lib.KIN_SPEED else
-                        ("velocity" if use_velocity else "head_direction")]
+            vec = self._agent_state()["measured_velocity" if self._variant == _lib.KIN_SPEED else
+                                      ("velocity" if use_velocity else "head_direction")]
             n_pos = ag.n_agents
         else:
-            if isinstance(vector, torch.Tensor):
-                vec = vector.to(device=self.device, dtype=torch.float64).reshape(-1, 2).contiguous()
-            else:
-                vec = torch.as_tensor(np.array(vector, dtype=np.float64).reshape(-1, 2), device=self.device)
-            if evaluate_at == "all":
-                n_pos = ag.Environment.flattened_discrete_coords.shape[0]
-            elif "pos" in kwargs:
-                n_pos = int(kwargs["pos"].reshape(-1, 2).shape[0]) if isinstance(kwargs["pos"], torch.Tensor) \
-                    else int(np.asarray(kwargs["pos"]).reshape(-1, 2).shape[0])
-            else:
-                n_pos = int(vec.shape[0])
+            vec = self._rows(vector)
+            n_pos = self._n_pos(evaluate_at, kwargs, int(vec.shape[0]))
             if vec.shape[0] not in (1, n_pos):
                 raise ValueError(f"{vec.shape[0]} direction / velocity vectors for {n_pos} positions: pass one (2,) vector "
                                  "or one per position")
@@ -1331,9 +1316,7 @@ class _KinematicCells(Neurons):
         out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
         _lib.check(self._lib.riab_kin_rates(vec.data_ptr(), per_position, n_pos, float(speed_scale), C.byref(c),
                                             out.data_ptr(), out.stride(0), ag._stream()))
-        if kwargs.get("return_tensor", False):
-            return out[:, : self.n]
-        return out[:, : self.n].T.contiguous().cpu().numpy().astype(np.float64)
+        return self._result(out, kwargs.get("return_tensor", False))
 
 
 class HeadDirectionCells(_KinematicCells):

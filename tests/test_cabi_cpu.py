@@ -245,7 +245,8 @@ def test_environment_mirror_polygon_and_holes_host_logic(golden):
 def test_mirror_default_params_match_the_reference():
     """Every default_params key of the reference's classes on the path exists in the host mirror with the same default
     (tests/golden/api_defaults.json, written from the live reference by oracle/gen_golden.py api); the mirror only ADDS
-    the batch-engine knobs."""
+    the batch-engine knobs.  Each mirror class descends from the same reference classes as in the reference
+    (ratinabox/Neurons.py:1259, 1535, 1892, 2151)."""
     import json
     import ratinabox_b200 as rb
     ref = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "api_defaults.json")))
@@ -279,10 +280,18 @@ def test_mirror_default_params_match_the_reference():
             assert k in have, (name, k)
             assert same(have[k], v), (name, k, have[k], v)
         extra = set(have) - set(want) - {"color"}
-        allowed = added.get(name, set()) | added["Neurons"] | {"dtheta", "name", "n", "min_fr", "max_fr"}
-        if name in ("Environment", "Agent"):
-            allowed = added.get(name, set())
-        assert extra <= allowed | set(ref.get("BoundaryVectorCells", {})), (name, sorted(extra - allowed))
+        allowed = added.get(name, set()) | (set() if name in ("Environment", "Agent") else added["Neurons"])
+        assert extra <= allowed, (name, sorted(extra - allowed))
+        assert ("dtheta" in have) == (name in ("BoundaryVectorCells", "FieldOfViewBVCs")), name
+
+    trees = {name: chain for name, (_, chain) in pairs.items()}
+    trees["AgentVectorCells"] = ["Neurons", "VectorCells", "AgentVectorCells"]
+    trees["FieldOfViewAVCs"] = trees["AgentVectorCells"] + ["FieldOfViewAVCs"]
+    ref_classes = {c for chain in trees.values() for c in chain}
+    for name, chain in trees.items():
+        assert [c.__name__ for c in reversed(getattr(rb, name).__mro__) if c.__name__ in ref_classes] == chain, name
+    for cls in (rb.ObjectVectorCells, rb.FieldOfViewOVCs, rb.AgentVectorCells, rb.FieldOfViewAVCs):
+        assert not issubclass(cls, rb.BoundaryVectorCells), cls.__name__
 
 
 def test_host_helpers_match_the_reference(golden):

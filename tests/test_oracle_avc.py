@@ -123,7 +123,7 @@ def test_mirror_default_params_match_the_reference(golden):
             assert k in have, (name, k)
             assert np.array_equal(np.asarray(have[k], dtype=object), np.asarray(v, dtype=object)), (name, k, have[k], v)
         extra = set(have) - set(want) - {"color"}
-        assert extra <= {"save_spikes", "history_bytes_limit", "dtheta"}, (name, sorted(extra))
+        assert extra <= {"save_spikes", "history_bytes_limit"}, (name, sorted(extra))
 
 
 def test_avc_pack_matches_numpy():
