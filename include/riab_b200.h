@@ -331,7 +331,9 @@ typedef struct {
  * (motion -> rates [-> noise] [-> spikes] -> history row).  `cells_kind` selects
  * which of pc / gc / bvc / ovc is read. */
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
-               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7 } riab_cells_kind;
+               RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7,
+               RIAB_CELLS_TD = 8 /* riab_td_cells: a FeedForwardLayer learning by TD (ValueNeuron, SuccessorFeatures) */
+} riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
   int64_t ld;
@@ -455,17 +457,58 @@ int riab_avc_rates(const double* pos_dev, int64_t n_pos, const double* other_pos
                    const riab_env* env, const riab_avc_cells* cells, const double* head_direction_dev, float* out_dev,
                    int64_t ld_out, void* stream);
 
+/* ------------------------------------------------ TD learning (RIAB_CELLS_TD)
+ * contribs/ValueNeuron.py:10-113 and contribs/SuccessorFeatures.py:12-49: a FeedForwardLayer whose update also keeps,
+ * per agent row,
+ *   deriv = (fr - fr_prev) / dt,  fr_prev <- fr                          (firingrate_deriv, ValueNeuron.py:66-71)
+ *   e_l   <- dt I_l + (1 - dt / tau_e) e_l   for every input l           (eligibility traces, :72-81)
+ * where I_l is the row the layer's contraction read (the layer's own new row for its self-recurrent input), and whose
+ * learning step (update_weights, :83-104) applies the mean over the rows of every row's reference update:
+ *   td   = reward + deriv - fr_prev / tau
+ *   W_l += dt eta (sum_a outer(td_a * phi'_a, e_{a,l}) / n_rows) - eta dt L2 W_l
+ * to float64 master weights, then rewrites the layer's W_hi | W_lo blocks (riab_ffl_pack of the new master, bit for
+ * bit).  The contraction runs over the row (agent) axis in fixed-size chunks whose float64 partial tiles are summed in
+ * a fixed order: no atomics, the same inputs give the same weights. */
+typedef struct {
+  riab_ffl_cells ffl;                       /* the layer; ffl.inputs[l].w_dev is the W_hi | W_lo block the learning rewrites */
+  float* fr_prev_dev;                       /* (A, ld) f32: firingrate of the last update (zeros before it and after reset) */
+  float* deriv_dev;                         /* (A, ld) f32 firingrate_deriv */
+  float* td_error_dev;                      /* (A, ld) f32 td_error (riab_td_reset zeroes it) */
+  int64_t ld;                               /* row stride of the layer's rates, fr_prev, deriv and td_error (floats) */
+  float* trace_dev[RIAB_FFL_MAX_INPUTS];    /* (A, trace_ld[l]) f32 eligibility trace of ffl.inputs[l] */
+  int64_t trace_ld[RIAB_FFL_MAX_INPUTS];    /* multiple of 4, >= ffl.inputs[l].n_in */
+  double* w_master_dev[RIAB_FFL_MAX_INPUTS];/* (n_cells, n_in) f64 row-major master weights of ffl.inputs[l] */
+  double dt, tau, tau_e, eta, L2;           /* Agent.dt and the ValueNeuron params; tau_e > 0 */
+  int32_t self_input;                       /* index of the input that is the layer itself (it reads fr_prev), or -1 */
+  int32_t reserved;
+} riab_td_cells;
+typedef enum { RIAB_TD_REWARD_SHARED = 0 /* (n_cells) f64, every row */, RIAB_TD_REWARD_ROWS = 1 /* (n_rows, ld) f32 */
+} riab_td_reward_mode;
+/* Number of agent chunks riab_td_learn splits the contraction of one input (n_in) into: float64 partial tiles of
+ * n_cells x n_in each, summed in a fixed order.  Depends on the shapes only. */
+int64_t riab_td_splits(int32_t n_cells, int32_t n_in, int64_t n_rows);
+/* Device scratch riab_td_learn needs for n_rows rows (bytes). */
+int64_t riab_td_scratch_bytes(const riab_td_cells* cells, int64_t n_rows);
+/* ValueNeuron.update_weights(reward) over n_rows rows: td -> td_error_out (n_rows, ld) f32, then every input's master
+ * and W_hi | W_lo.  scratch: riab_td_scratch_bytes device bytes, 16-byte aligned. */
+int riab_td_learn(const riab_td_cells* cells, int64_t n_rows, const void* reward, int32_t reward_mode, float* td_error_out,
+                  void* scratch, void* stream);
+/* ValueNeuron.reset (:106-113): zero fr_prev, deriv, td_error and the traces of the rows whose mask byte is non-zero
+ * (mask (A) uint8 device, NULL = every row). */
+int riab_td_reset(const riab_td_cells* cells, int64_t n_rows, const uint8_t* mask, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
  * Population 0 is fused with the motion kernel, the others use riab_neurons_update; FeedForwardLayers
- * (RIAB_CELLS_FFL) run after every other population of the step, in index order, reading ring rows
- * (next + s - lag) of their inputs, and an Agent with one keeps this unskewed schedule.
+ * (RIAB_CELLS_FFL, and RIAB_CELLS_TD with its trace pass) run after every other population of the step, in index order,
+ * reading ring rows (next + s - lag) of their inputs, and an Agent with one keeps this unskewed schedule.  A TD layer's
+ * self-recurrent input reads its fr_prev.  riab_run never calls riab_td_learn.
  * History rows go to device rings: row (next + s) % rows for step s. */
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
-                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* */
+                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

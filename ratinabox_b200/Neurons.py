@@ -1074,6 +1074,10 @@ class FeedForwardLayer(Neurons):
         c.n_inputs = len(self.inputs)
         return c
 
+    def _layer_struct(self, c):
+        """The riab_ffl_cells part of the struct _cells() returns."""
+        return c
+
     def _slot_ptr(self, layer, slot):
         if slot is None:
             return None                   # never updated: the reference's initial zeros (Neurons.py:120)
@@ -1134,7 +1138,7 @@ class FeedForwardLayer(Neurons):
         if evaluate_at == "last":
             self.Agent._flush_pending()
             n_pos = self.Agent.n_agents
-            fc = c
+            fc = self._layer_struct(c)
         else:
             fc = _lib.FflCells.from_buffer_copy(c)
             fc.prime_dev = None

@@ -99,6 +99,20 @@ class FflCells(C.Structure):
                 ("inputs", FflInput * FFL_MAX_INPUTS)]
 
 
+class TdCells(C.Structure):
+    _fields_ = [("ffl", FflCells), ("fr_prev_dev", C.c_void_p), ("deriv_dev", C.c_void_p), ("td_error_dev", C.c_void_p),
+                ("ld", C.c_int64), ("trace_dev", C.c_void_p * FFL_MAX_INPUTS), ("trace_ld", C.c_int64 * FFL_MAX_INPUTS),
+                ("w_master_dev", C.c_void_p * FFL_MAX_INPUTS), ("dt", C.c_double), ("tau", C.c_double),
+                ("tau_e", C.c_double), ("eta", C.c_double), ("L2", C.c_double), ("self_input", C.c_int32),
+                ("reserved", C.c_int32)]
+    # FeedForwardLayer's host code reaches the embedded layer's fields through these (they share the struct's memory)
+    inputs = property(lambda self: self.ffl.inputs)
+    prime_dev = property(lambda self: self.ffl.prime_dev, lambda self, v: setattr(self.ffl, "prime_dev", v))
+
+
+TD_REWARD_SHARED, TD_REWARD_ROWS = 0, 1                       # riab_td_reward_mode
+
+
 class RsnCells(C.Structure):
     _fields_ = [("points", PlaceCells), ("targets_dev", C.c_void_p), ("n_cells", C.c_int32), ("n_points", C.c_int32),
                 ("k_pad", C.c_int32), ("min_fr", C.c_float), ("max_fr", C.c_float), ("reserved", C.c_int32)]
@@ -146,7 +160,7 @@ class AgentHistory(C.Structure):
 PC_DESCRIPTIONS = {"gaussian": 0, "gaussian_threshold": 1, "diff_of_gaussians": 2, "top_hat": 3, "one_hot": 4}
 WALL_GEOMETRIES = {"euclidean": 0, "line_of_sight": 1, "geodesic": 2}
 GC_DESCRIPTIONS = {"rectified_cosines": 0, "shifted_cosines": 1}
-CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL, CELLS_RSN, CELLS_KIN, CELLS_AVC = 0, 1, 2, 3, 4, 5, 6, 7
+CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL, CELLS_RSN, CELLS_KIN, CELLS_AVC, CELLS_TD = 0, 1, 2, 3, 4, 5, 6, 7, 8
 KIN_HEAD_DIRECTION, KIN_VELOCITY, KIN_SPEED = 0, 1, 2                # riab_kin_variant
 PLACE_MAX_WI = 8                                              # inner walls of the line-of-sight / geodesic kernels
 ACTIVATIONS = {"linear": 0, "sigmoid": 1, "relu": 2, "tanh": 3, "retanh": 4, "softmax": 5}   # riab_activation
@@ -186,6 +200,10 @@ SYMBOLS = {
     "riab_ffl_pack": (C.c_int, [c_double_p, C.c_int32, C.c_int32, C.POINTER(FflInput), c_float_p]),
     "riab_ffl_rates": (C.c_int, [C.POINTER(FflCells), C.c_int64, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut),
                                  C.c_void_p]),
+    "riab_td_splits": (C.c_int64, [C.c_int32, C.c_int32, C.c_int64]),
+    "riab_td_scratch_bytes": (C.c_int64, [C.POINTER(TdCells), C.c_int64]),
+    "riab_td_learn": (C.c_int, [C.POINTER(TdCells), C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "riab_td_reset": (C.c_int, [C.POINTER(TdCells), C.c_int64, C.c_void_p, C.c_void_p]),
     "riab_rsn_pack_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "riab_rsn_pack": (C.c_int, [c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_double, c_double_p, C.c_int32, C.c_int32,
                                 c_double_p, C.c_int32, C.POINTER(RsnCells), c_float_p, c_double_p]),

@@ -1,1 +1,3 @@
 from .TaskEnvironment import SpatialGoalEnvironment  # noqa: F401
+from .ValueNeuron import ValueNeuron  # noqa: F401
+from .SuccessorFeatures import SuccessorFeatures  # noqa: F401

@@ -11,6 +11,7 @@
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
 //   k_bvc_rays<TABLE>   BVC phase A (float64 rays)
 //   k_bvc_integrate     BVC phase B (float32 angular integral, TMA-staged tables)
+//   k_td_*              TD learning of ValueNeuron / SuccessorFeatures (riab_td.cuh)
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -31,6 +32,7 @@
 #include "riab_place.cuh"
 #include "riab_rsn.cuh"
 #include "riab_traj.cuh"
+#include "riab_td.cuh"
 
 using namespace riab;
 
@@ -2028,6 +2030,76 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
 }
 
 // ---------------------------------------------------------------------------
+// TD learning (riab_td.cuh).  check_td: the TD state of a layer whose riab_ffl_cells part check_ffl already accepted.
+int check_td(const riab_td_cells* t, long long out_ld) {
+  if (t == nullptr) return fail(RIAB_ERR_INVALID, "td cells NULL");
+  const riab_ffl_cells& f = t->ffl;
+  if (t->fr_prev_dev == nullptr || t->deriv_dev == nullptr || t->td_error_dev == nullptr)
+    return fail(RIAB_ERR_INVALID, "td: fr_prev / deriv / td_error NULL");
+  if (t->ld != out_ld || t->ld % 4 != 0 || t->ld < f.n_cells)
+    return fail(RIAB_ERR_INVALID, "td: ld %lld must equal the rates' ld (%lld), a multiple of 4", (long long)t->ld, out_ld);
+  if (!(t->dt > 0.0) || !(t->tau_e > 0.0) || !std::isfinite(t->tau_e) || !std::isfinite(t->dt))
+    return fail(RIAB_ERR_INVALID, "td: dt and tau_e must be finite and > 0");
+  if (t->self_input < -1 || t->self_input >= f.n_inputs) return fail(RIAB_ERR_INVALID, "td: bad self_input %d", t->self_input);
+  if (f.n_inputs < 0 || f.n_inputs > RIAB_FFL_MAX_INPUTS) return fail(RIAB_ERR_UNSUPPORTED, "td: %d inputs", f.n_inputs);
+  for (int l = 0; l < f.n_inputs; ++l) {
+    const riab_ffl_input& in = f.inputs[l];
+    if (t->trace_dev[l] == nullptr || t->w_master_dev[l] == nullptr || in.w_dev == nullptr || in.n_in <= 0 ||
+        in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK)
+      return fail(RIAB_ERR_INVALID, "td input %d: trace / master / packed weights missing or mis-sized", l);
+    if (t->trace_ld[l] < in.n_in || t->trace_ld[l] % 4 != 0 || ((uintptr_t)t->trace_dev[l]) % 16 != 0)
+      return fail(RIAB_ERR_INVALID, "td input %d: trace rows must be 16-byte aligned with ld >= n_in, a multiple of 4", l);
+  }
+  return 0;
+}
+
+// k_td_trace over n_rows rows after the layer's rates (checked by check_ffl / check_td)
+int launch_td_trace(const riab_td_cells* t, long long n_rows, const float* rates, cudaStream_t s) {
+  if (n_rows == 0) return 0;
+  TdTraceK k;
+  memset(&k, 0, sizeof(k));
+  k.rates = rates; k.fr_prev = t->fr_prev_dev; k.deriv = t->deriv_dev;
+  k.ld = t->ld; k.n_rows = n_rows; k.n_cells = t->ffl.n_cells; k.n_inputs = t->ffl.n_inputs;
+  for (int l = 0; l < k.n_inputs; ++l) {
+    const riab_ffl_input& in = t->ffl.inputs[l];
+    const bool self = l == t->self_input;              // ValueNeuron.update reads the layer's NEW firingrate
+    k.in[l] = self ? rates : in.rows_dev;
+    k.in_ld[l] = self ? t->ld : in.ld;
+    k.trace[l] = t->trace_dev[l]; k.trace_ld[l] = t->trace_ld[l]; k.n_in[l] = in.n_in;
+  }
+  k.dt = (float)t->dt;
+  k.decay = (float)(1.0 - t->dt / t->tau_e);
+  k_td_trace<<<(unsigned)n_rows, TD_TRACE_THREADS, 0, s>>>(k);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// The split of the agent axis of one learning contraction: from the shapes alone (so the same shapes always sum in the
+// same order), about TD_TARGET_CTAS CTAs (16 per SM for the bandwidth-bound 8-row tiles, whose loads need the CTAs in
+// flight; 4 per SM for the 64 x 64 tiles), chunks a multiple of TD_KC agents.
+constexpr int TD_TARGET_CTAS = 4 * 132, TD_TARGET_CTAS_SMALL = 16 * 132;
+struct TdSplit {
+  bool small = false;            // n <= 8: one 8-row CUDA-core tile (8 x 256), else 64 x 64 wgmma tiles
+  int tiles = 0;
+  long long chunk = 0, splits = 0;
+};
+TdSplit td_split(int n, int n_in, long long A) {
+  TdSplit t;
+  t.small = n <= 8;
+  const int bm = t.small ? 8 : 64, bn = t.small ? 256 : 64;
+  t.tiles = ((n + bm - 1) / bm) * ((n_in + bn - 1) / bn);
+  const long long rounds = (A + TD_KC - 1) / TD_KC;
+  const int target = t.small ? TD_TARGET_CTAS_SMALL : TD_TARGET_CTAS;
+  const long long want = std::max(1LL, std::min(rounds, (long long)((target + t.tiles - 1) / t.tiles)));
+  t.chunk = (rounds + want - 1) / want * TD_KC;
+  t.splits = (A + t.chunk - 1) / t.chunk;
+  return t;
+}
+long long td_g_ld(int n) { return (n + 7) / 8 * 8; }
+size_t td_g_bytes(int n, long long A) { return ((size_t)A * td_g_ld(n) * 4 + 255) / 256 * 256; }
+
+// ---------------------------------------------------------------------------
 // RandomSpatialNeurons (riab_rsn.cuh).  The sample points are a place-cell population: make_place validates them and
 // sets up their constants, in the direct (not expanded) Gaussian form with the [0, 1] scale.
 int make_rsn(const riab_rsn_cells* r, const EnvK& env, PlaceConst& c) {
@@ -2135,6 +2207,7 @@ struct Pop {
   PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
+  const riab_td_cells* td = nullptr;    // RIAB_CELLS_TD: its layer is `ffl`
   const riab_rsn_cells* rsn = nullptr;  // its sample points: `place`
 };
 
@@ -2162,6 +2235,10 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   } else if (kind == RIAB_CELLS_FFL) {
     d.ffl = (const riab_ffl_cells*)cells;
     d.n_cells = d.ffl->n_cells;
+  } else if (kind == RIAB_CELLS_TD) {
+    d.td = (const riab_td_cells*)cells;
+    d.ffl = &d.td->ffl;
+    d.n_cells = d.ffl->n_cells;
   } else if (kind == RIAB_CELLS_RSN) {
     d.rsn = (const riab_rsn_cells*)cells;
     rc = make_rsn(d.rsn, ek, d.place);
@@ -2177,8 +2254,12 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   }
   if (rc || (rc = make_out(out, noise, d.n_cells, dt, ag.id_offset, d.out, d.bound))) return rc;
   if (kind == RIAB_CELLS_BVC) return check_bvc(ek, d.bvc, d.bvc_scratch = out->bvc_scratch, ag.n_agents);
+  if (kind == RIAB_CELLS_TD) return (rc = check_ffl(d.ffl, d.out, ag.n_agents)) ? rc : check_td(d.td, d.out.ld);
   return kind == RIAB_CELLS_FFL ? check_ffl(d.ffl, d.out, ag.n_agents) : 0;
 }
+
+// FeedForwardLayer-like kinds: they read other populations' rows and run after them (plan_run)
+bool ffl_like(int kind) { return kind == RIAB_CELLS_FFL || kind == RIAB_CELLS_TD; }
 
 // One population's kernels for one step.  MODE 0: rates at the agents' positions; 1: the motion step fused in; 2: skewed
 // (rates at the current positions while the motion of the next step runs, riab_run).  BVC, FFL and RSN populations run
@@ -2196,7 +2277,8 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
     if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, ag.n_agents, d.out, s);
-    return launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
+    const int rc = launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
+    return (rc || d.kind != RIAB_CELLS_TD) ? rc : launch_td_trace(d.td, ag.n_agents, d.out.rates, s);
   } else {
     return fail(RIAB_ERR_INVALID, "cells kind %d is launched unfused", d.kind);
   }
@@ -2208,7 +2290,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
 // RandomSpatialNeurons (a GEMM kernel without motion warps).
 bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
   return io.collision_mask || io.first_hit || io.n_iters || d.kind == RIAB_CELLS_BVC || d.kind == RIAB_CELLS_FFL ||
-         d.kind == RIAB_CELLS_RSN ||
+         d.kind == RIAB_CELLS_TD || d.kind == RIAB_CELLS_RSN ||
          (d.kind == RIAB_CELLS_PLACE && d.place.desc == RIAB_PC_ONE_HOT);
 }
 
@@ -2362,7 +2444,7 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   // A FeedForwardLayer reads other populations' rows of the same step and masks the agents whose position of that step is
   // NaN, so an Agent with one keeps the plain schedule: the positions advance before any population of the step.
   bool any_ffl = false;
-  for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || pops[p].kind == RIAB_CELLS_FFL;
+  for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || ffl_like(pops[p].kind);
   const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
                        ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
   // Skewed schedule (population 0 is a Place / Grid / OVC / kinematic / AVC population): motion(0) alone, then per step one kernel that
@@ -2373,14 +2455,14 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
                     io.xi == nullptr &&
                     !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr;
   plan.sched = skew ? RunPlan::SKEWED : RunPlan::PLAIN;
-  plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || pops[0].kind == RIAB_CELLS_FFL);
+  plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || ffl_like(pops[0].kind));
   // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
   // FeedForwardLayers in registration order, after every row they read of this step exists
   for (int p = skew ? 1 : 0; p < n_pops; ++p)
-    if (pops[p].kind != RIAB_CELLS_FFL) plan.order.push_back(p);
+    if (!ffl_like(pops[p].kind)) plan.order.push_back(p);
   if (skew) plan.order.push_back(0);
   for (int p = 0; p < n_pops; ++p)
-    if (pops[p].kind == RIAB_CELLS_FFL) plan.order.push_back(p);
+    if (ffl_like(pops[p].kind)) plan.order.push_back(p);
   return 0;
 }
 
@@ -2454,11 +2536,20 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
       ro.rates_row = pp.rates_ring; ro.spikes_row = pp.spikes_ring;
       riab_neuron_noise nz = pp.noise;
       nz.step = pp.noise.step + (uint64_t)st; nz.dt = prm->dt;
-      riab_ffl_cells fc;
-      if (pp.kind == RIAB_CELLS_FFL) {
+      riab_td_cells tc;                             // an FFL population uses tc.ffl only
+      riab_ffl_cells& fc = tc.ffl;
+      const void* cells = pp.cells;
+      if (ffl_like(pp.kind)) {
         // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
         // previous step's: before the first step, the row the caller passed
-        fc = *(const riab_ffl_cells*)pp.cells;
+        if (pp.kind == RIAB_CELLS_TD) {
+          if (pp.cells == nullptr) return fail(RIAB_ERR_INVALID, "population %d: cells NULL", p);
+          tc = *(const riab_td_cells*)pp.cells;
+          cells = &tc;
+        } else {
+          fc = *(const riab_ffl_cells*)pp.cells;
+          cells = &fc;
+        }
         for (int i = 0; i < fc.n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
           riab_ffl_input& in = fc.inputs[i];
           if (in.population < 0 || in.population >= n_pops || (in.lag == 0) != (in.population < p) || in.lag < 0 || in.lag > 1)
@@ -2471,10 +2562,13 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
           in.rows_dev = ring_row(ip.rates_ring, ip.ring_next + st - in.lag, ip.ring_rows, A * ip.out.ld);
           in.ld = ip.out.ld;
         }
+        if (pp.kind == RIAB_CELLS_TD && tc.self_input >= 0 && tc.self_input < fc.n_inputs) {
+          fc.inputs[tc.self_input].rows_dev = tc.fr_prev_dev;       // firingrate_last, as in the stepped update
+          fc.inputs[tc.self_input].ld = tc.ld;
+        }
       }
       Pop d;
-      if ((rc = make_pop(ek, pp.kind, pp.kind == RIAB_CELLS_FFL ? (const void*)&fc : pp.cells, &ro, &nz, prm->dt, *agents, d)))
-        return rc;
+      if ((rc = make_pop(ek, pp.kind, cells, &ro, &nz, prm->dt, *agents, d))) return rc;
       d.out.rates = ring_row(pp.rates_ring, pp.ring_next + st, pp.ring_rows, A * pp.out.ld);
       if (d.out.spikes != nullptr) d.out.spikes = ring_row(pp.spikes_ring, pp.ring_next + st, pp.ring_rows, A * d.out.spike_ld);
       if (p != 0 || plan.motion_alone) rc = launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s, pipe.pipe);
@@ -2977,6 +3071,101 @@ int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_
   if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
       (rc = check_ffl(ffl, ok, n_rows))) return rc;
   return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------ TD learning
+int64_t riab_td_splits(int32_t n_cells, int32_t n_in, int64_t n_rows) {
+  if (n_cells <= 0 || n_in <= 0 || n_rows < 0) {
+    fail(RIAB_ERR_INVALID, "riab_td_splits: bad argument");
+    return -1;
+  }
+  return td_split(n_cells, n_in, n_rows).splits;
+}
+
+int64_t riab_td_scratch_bytes(const riab_td_cells* t, int64_t n_rows) {
+  if (t == nullptr || n_rows < 0 || t->ffl.n_cells <= 0 || t->ffl.n_inputs < 0 || t->ffl.n_inputs > RIAB_FFL_MAX_INPUTS) {
+    fail(RIAB_ERR_INVALID, "riab_td_scratch_bytes: bad argument");
+    return -1;
+  }
+  size_t part = 0;
+  for (int l = 0; l < t->ffl.n_inputs; ++l) {
+    const int n_in = t->ffl.inputs[l].n_in;
+    if (n_in <= 0) { fail(RIAB_ERR_INVALID, "riab_td_scratch_bytes: input %d has n_in %d", l, n_in); return -1; }
+    const TdSplit sp = td_split(t->ffl.n_cells, n_in, n_rows);
+    part = std::max(part, (size_t)sp.splits * t->ffl.n_cells * n_in * sizeof(double));
+  }
+  return (int64_t)(td_g_bytes(t->ffl.n_cells, n_rows) + part);
+}
+
+int riab_td_learn(const riab_td_cells* t, int64_t n_rows, const void* reward, int32_t reward_mode, float* td_error_out,
+                  void* scratch, void* stream) {
+  if (t == nullptr || n_rows < 0 || reward == nullptr || td_error_out == nullptr || scratch == nullptr ||
+      (reward_mode != RIAB_TD_REWARD_SHARED && reward_mode != RIAB_TD_REWARD_ROWS))
+    return fail(RIAB_ERR_INVALID, "riab_td_learn: bad argument");
+  if (((uintptr_t)scratch) % 16 != 0) return fail(RIAB_ERR_INVALID, "riab_td_learn: scratch must be 16-byte aligned");
+  int rc;
+  if ((rc = check_td(t, t->ld))) return rc;
+  const riab_ffl_cells& f = t->ffl;
+  if (f.prime_dev == nullptr) return fail(RIAB_ERR_INVALID, "riab_td_learn: prime_dev NULL");
+  if (n_rows == 0) return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int n = f.n_cells;
+  TdGK g;
+  g.fr = t->fr_prev_dev; g.deriv = t->deriv_dev; g.prime = f.prime_dev;
+  g.reward_shared = reward_mode == RIAB_TD_REWARD_SHARED ? (const double*)reward : nullptr;
+  g.reward_rows = reward_mode == RIAB_TD_REWARD_ROWS ? (const float*)reward : nullptr;
+  g.td = td_error_out;
+  g.g = (float*)scratch;
+  g.ld = t->ld; g.ldg = td_g_ld(n); g.n_rows = n_rows; g.n_cells = n;
+  g.inv_tau = 1.0 / t->tau;
+  const long long ng = n_rows * g.ldg;
+  k_td_g<<<(unsigned)((ng + 255) / 256), 256, 0, s>>>(g);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  double* part = (double*)((char*)scratch + td_g_bytes(n, n_rows));
+  for (int l = 0; l < f.n_inputs; ++l) {
+    const riab_ffl_input& in = f.inputs[l];
+    const TdSplit sp = td_split(n, in.n_in, n_rows);
+    TdLearnK lk;
+    lk.g = g.g; lk.e = t->trace_dev[l]; lk.part = part;
+    lk.ldg = g.ldg; lk.lde = t->trace_ld[l]; lk.n_rows = n_rows; lk.chunk = sp.chunk;
+    lk.n_cells = n; lk.n_in = in.n_in;
+    const dim3 grid((unsigned)sp.tiles, (unsigned)sp.splits);
+    if (sp.small) k_td_learn<8, 256, 8, 1><<<grid, TD_THREADS, 0, s>>>(lk);
+    else k_td_learn_tc<<<grid, TD_TC_THREADS, 0, s>>>(lk);
+    g_launches++;
+    RIAB_CUDA_OK(cudaGetLastError());
+    TdApplyK ak;
+    ak.part = part; ak.w = t->w_master_dev[l];
+    ak.whi = const_cast<float*>(in.w_dev);
+    ak.wlo = ak.whi + (size_t)((n + 7) / 8 * 8) * in.k_pad;
+    ak.n_cells = n; ak.n_in = in.n_in; ak.k_pad = in.k_pad; ak.splits = (int)sp.splits;
+    ak.n_rows = (double)n_rows;
+    ak.c_grad = t->dt * t->eta;                       // self.Agent.dt * self.eta
+    ak.c_decay = t->eta * t->dt * t->L2;              // self.eta * self.Agent.dt * self.L2
+    const long long nw = (long long)n * in.n_in;
+    if (sp.splits >= 32) k_td_apply<true><<<(unsigned)((32 * nw + 255) / 256), 256, 0, s>>>(ak);
+    else k_td_apply<false><<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(ak);
+    g_launches++;
+    RIAB_CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
+
+int riab_td_reset(const riab_td_cells* t, int64_t n_rows, const uint8_t* mask, void* stream) {
+  if (t == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_td_reset: bad argument");
+  int rc;
+  if ((rc = check_td(t, t->ld))) return rc;
+  if (n_rows == 0) return 0;
+  TdResetK k;
+  memset(&k, 0, sizeof(k));
+  k.rows[0] = t->fr_prev_dev; k.rows[1] = t->deriv_dev; k.rows[2] = t->td_error_dev;
+  k.ld = t->ld; k.n_rows = n_rows; k.n_inputs = t->ffl.n_inputs; k.mask = mask;
+  for (int l = 0; l < k.n_inputs; ++l) { k.trace[l] = t->trace_dev[l]; k.trace_ld[l] = t->trace_ld[l]; }
+  k_td_reset<<<(unsigned)n_rows, 128, 0, (cudaStream_t)stream>>>(k);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
 }
 
 // ------------------------------------------------------- RandomSpatialNeurons
