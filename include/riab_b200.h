@@ -332,7 +332,8 @@ typedef struct {
  * which of pc / gc / bvc / ovc is read. */
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
                RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7,
-               RIAB_CELLS_TD = 8 /* riab_td_cells: a FeedForwardLayer learning by TD (ValueNeuron, SuccessorFeatures) */
+               RIAB_CELLS_TD = 8 /* riab_td_cells: a FeedForwardLayer learning by TD (ValueNeuron, SuccessorFeatures) */,
+               RIAB_CELLS_PPPC = 9 /* riab_pppc_cells: PhasePrecessingPlaceCells */
 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
@@ -497,6 +498,25 @@ int riab_td_learn(const riab_td_cells* cells, int64_t n_rows, const void* reward
  * (mask (A) uint8 device, NULL = every row). */
 int riab_td_reset(const riab_td_cells* cells, int64_t n_rows, const uint8_t* mask, void* stream);
 
+/* ------------------------------------ PhasePrecessingPlaceCells (RIAB_CELLS_PPPC)
+ * contribs/PhasePrecessingPlaceCells.py:66-119: at the agents, the PlaceCells rate of `place` times the theta modulation
+ *   factor_i = von_mises(pi - s_i precess_fraction pi - phi, 0, sigma) 2 pi = exp(kappa cos x) / I0(kappa), kappa = 1/sigma^2
+ *   phi = theta_freq (t % (1 / theta_freq)) 2 pi,  s_i = ((pos - c_i) . d) / sigma_i,  d = velocity / (1e-8 + |velocity|)
+ *   sigma_i = the cell's width (riab_place_pack's widths), times 2 for "gaussian"
+ * Rates are not bounded by max_fr (the factor peaks at exp(kappa) / I0(kappa)).  one_hot is refused. */
+typedef struct {
+  riab_place_cells place;        /* riab_place_pack of place_cell_centres / place_cell_widths; description != one_hot */
+  double theta_freq;             /* Hz */
+  double sigma;                  /* the von Mises spread sqrt(1 / kappa), as the reference stores it at construction */
+  double precess_fraction;
+  double t;                      /* Agent.t of the step (after its `t += dt`); riab_run: of the first step, the library
+                                    advances it by `t += dt` per step */
+} riab_pppc_cells;
+/* PhasePrecessingPlaceCells.get_state(evaluate_at="agent"): pos_dev / velocity_dev (n_pos,2) f64, the agents' positions
+ * and Agent.velocity -> out_dev (n_pos, ld_out) f32.  No noise, no NaN-position masking. */
+int riab_pppc_rates(const double* pos_dev, const double* velocity_dev, int64_t n_pos, const riab_env* env,
+                    const riab_pppc_cells* cells, float* out_dev, int64_t ld_out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
@@ -508,7 +528,7 @@ int riab_td_reset(const riab_td_cells* cells, int64_t n_rows, const uint8_t* mas
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
-                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* */
+                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* / riab_pppc_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

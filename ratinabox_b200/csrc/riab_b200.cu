@@ -5,7 +5,7 @@
 //   k_agent_update_src  Agent.update from an imported trajectory / forced positions, one agent per thread (float64)
 //   k_traj_build        not-a-knot spline of imported trajectories, one thread per (trajectory, axis) column
 //   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells / ObjectVectorCells /
-//                       head direction, velocity and speed cells / AgentVectorCells:
+//                       head direction, velocity and speed cells / AgentVectorCells / PhasePrecessingPlaceCells:
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
@@ -30,6 +30,7 @@
 #include "riab_kin.cuh"
 #include "riab_motion.cuh"
 #include "riab_place.cuh"
+#include "riab_pppc.cuh"
 #include "riab_rsn.cuh"
 #include "riab_traj.cuh"
 #include "riab_td.cuh"
@@ -491,6 +492,44 @@ struct AvcPolicy {
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const&) { return 0; }
+};
+
+// PhasePrecessingPlaceCells: PlacePolicy's record, cells and rates (direct exponent form), times the theta modulation
+// factor of riab_pppc.cuh.  MODE 0 reads the rows' velocities from Const::vel (given_dir: the one given vector stands for
+// every kinematic input).
+template <int WI, int DESC>
+struct PppcPolicy {
+  using Place = PlacePolicy<WI, DESC>;
+  using Const = PppcConst;
+  using Regs = PppcCellRegs<WI>;
+  static constexpr int REC = pppc_rec(WI);
+  static constexpr bool LIGHT = false;    // ~10 more instructions per rate and 12 more cell registers than PlacePolicy
+  static constexpr bool THIN = false;     // the factor has no a-priori bound below M max_fr: dense spike stream
+  static constexpr bool POSITIONAL = true;
+  static __device__ __forceinline__ void given_dir(const Const& c, long long i, double& x, double& y) {
+    if (c.vel != nullptr) { x = c.vel[2 * i]; y = c.vel[2 * i + 1]; }
+  }
+  static __device__ __forceinline__ void prepare(double* aux, const double* s_walls, const Const& c) {
+    Place::prepare(aux, s_walls, c);
+  }
+  static __device__ __forceinline__ void record(float* rec, long long i, double px, double py, double hdx, double hdy,
+                                                double vx, double vy, double mvx, double mvy, const double* s_walls,
+                                                const double* aux, const Const& c, const EnvK& env) {
+    Place::record(rec, i, px, py, hdx, hdy, vx, vy, mvx, mvy, s_walls, aux, c, env);
+    pppc_direction_record(rec + pppc_dir(WI), px, py, vx, vy, env.cxm, env.cym);
+  }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) {
+    Place::load(r.p, c, cell0);
+    pppc_load_phase<WI>(r, c);
+  }
+  template <bool DEFER, int EXP = -1>
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int cell0,
+                                                const float* rec, uint32_t inner_s, bool& unsure) {
+    Place::template rates4<DEFER, 0>(o, r.p, c, cell0, rec, inner_s, unsure);
+    pppc_modulate4<WI>(o, r, c, rec + pppc_dir(WI));
+  }
+  static __device__ __forceinline__ int expanded(const Const&) { return 0; }
+  static __device__ __forceinline__ int wall0(const Const& c) { return c.wall0; }
 };
 
 // ---------------------------------------------------------------------------
@@ -1731,6 +1770,37 @@ int make_avc(const riab_avc_cells* vc, const EnvK& env, const double* head_dir, 
   return 0;
 }
 
+// PhasePrecessingPlaceCells at the clock pc->t: the place constants in their direct form, and the launch's theta phase
+// and von Mises constants in float64, in the reference's operation order (PhasePrecessingPlaceCells.py:100-117,
+// utils.py:452-456).  vel: the rows' velocities.
+int make_pppc(const riab_pppc_cells* pc, const EnvK& env, const double* vel, PppcConst& c) {
+  if (pc == nullptr) return fail(RIAB_ERR_INVALID, "phase precessing place cells NULL");
+  memset(&c, 0, sizeof(c));
+  int rc;
+  if ((rc = make_place(&pc->place, env, c))) return rc;
+  if (pc->place.description == RIAB_PC_ONE_HOT)
+    return fail(RIAB_ERR_INVALID, "phase precessing place cells need a description with widths (not one_hot)");
+  if (!(std::isfinite(pc->theta_freq) && pc->theta_freq != 0.0) || !(std::isfinite(pc->sigma) && pc->sigma > 0.0) ||
+      !std::isfinite(pc->precess_fraction) || !std::isfinite(pc->t))
+    return fail(RIAB_ERR_INVALID, "phase precessing place cells: theta_freq %g, sigma %g, precess_fraction %g, t %g",
+                pc->theta_freq, pc->sigma, pc->precess_fraction, pc->t);
+  c.expanded = 0; c.fold = 0; c.lspan = 0.f;                          // the direct form of the DESC = -1 kernels
+  const double period = 1.0 / pc->theta_freq;
+  double r = fmod(pc->t, period);                                      // Python's t % period: the sign of the divisor
+  if (r != 0.0 && ((r < 0.0) != (period < 0.0))) r += period;
+  const double phi = pc->theta_freq * r * 2.0 * M_PI;
+  c.u = (float)((M_PI - phi) / (2.0 * M_PI));
+  const double kappa = 1.0 / (pc->sigma * pc->sigma);
+  double norm = exp(kappa) / (2.0 * M_PI * std::cyl_bessel_i(0.0, kappa));
+  norm = norm / exp(kappa);
+  c.k2 = (float)(kappa * 1.4426950408889634);
+  c.lnorm = (float)log2(norm * 2.0 * M_PI);
+  const double m = (pc->place.description == RIAB_PC_GAUSSIAN) ? 2.0 : 1.0;   // gaussian fields end at 2 sigma (:104-105)
+  c.gs = pc->precess_fraction / (2.0 * m) * sqrt(2.0 / 1.4426950408889634);
+  c.vel = vel;
+  return 0;
+}
+
 int g_num_sms = 0;
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
@@ -1839,6 +1909,19 @@ int launch_place(const EnvK& env, const riab_agents& ag, const riab_motion_param
   if (pc.desc == RIAB_PC_GAUSSIAN && pc.geometry != RIAB_GEOM_GEODESIC)
     return launch_place_d<MODE, RIAB_PC_GAUSSIAN>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
   return launch_place_d<MODE, -1>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+}
+
+// PhasePrecessingPlaceCells: the run-time description profile only, MODE 0 / 1 / 2 (no whole run)
+template <int MODE>
+int launch_pppc(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
+                const PppcConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s) {
+  static_assert(MODE <= 2, "phase precessing place cells have no whole-run launch");
+  const int wi = pc.n_inner;
+  if (wi == 0) return launch_tile<PppcPolicy<0, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  if (wi == 1) return launch_tile<PppcPolicy<1, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  if (wi == 2) return launch_tile<PppcPolicy<2, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  if (wi <= 4) return launch_tile<PppcPolicy<4, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  return launch_tile<PppcPolicy<8, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
 }
 
 // riab_run pipelines BoundaryVectorCells across steps: the float64 ray kernel of step s+1 (latency-bound, FP64 pipe) runs
@@ -2204,7 +2287,7 @@ struct Pop {
   int kind = -1, n_cells = 0;
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
-  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc;
+  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc; PppcConst pppc;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
   const riab_td_cells* td = nullptr;    // RIAB_CELLS_TD: its layer is `ffl`
@@ -2249,6 +2332,9 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   } else if (kind == RIAB_CELLS_AVC) {
     rc = make_avc((const riab_avc_cells*)cells, ek, ag.head_direction, ag.n_agents, d.avc);
     d.n_cells = d.avc.n_cells;
+  } else if (kind == RIAB_CELLS_PPPC) {
+    rc = make_pppc((const riab_pppc_cells*)cells, ek, ag.velocity, d.pppc);
+    d.n_cells = ((const riab_pppc_cells*)cells)->place.n_cells;
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
@@ -2273,6 +2359,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
   if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_PPPC) return launch_pppc<MODE>(ek, ag, mp, io, d.pppc, d.out, pos_in, ag.n_agents, s);
   if constexpr (MODE == 0) {
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
@@ -2318,7 +2405,8 @@ int neurons_update_impl(bool fused, const riab_agents* agents, const riab_env* e
 
 // get_state: the rates at n_pos given positions (and head directions, egocentric cells), without noise or spikes
 int rates_at(int kind, const void* cells, const double* pos_dev, int64_t n_pos, const riab_env* env, const double* head_dir,
-             float* scratch, int32_t* first_wall, float* out_dev, int64_t ld_out, void* stream) {
+             float* scratch, int32_t* first_wall, float* out_dev, int64_t ld_out, void* stream,
+             const double* velocity = nullptr) {
   if (n_pos == 0) return 0;
   EnvK ek;
   Pop d;
@@ -2328,7 +2416,7 @@ int rates_at(int kind, const void* cells, const double* pos_dev, int64_t n_pos, 
   riab_rates_out ro = {};
   ro.rates_row = out_dev; ro.ld = ld_out; ro.bvc_scratch = scratch;
   riab_agents at = {};
-  at.n_agents = n_pos; at.pos = (double*)pos_dev; at.head_direction = (double*)head_dir;
+  at.n_agents = n_pos; at.pos = (double*)pos_dev; at.head_direction = (double*)head_dir; at.velocity = (double*)velocity;
   if ((rc = make_pop(ek, kind, cells, &ro, nullptr, 1.0, at, d))) return rc;
   d.first_wall = first_wall;
   return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
@@ -2517,6 +2605,10 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
   }
   PipeScope pipe;
   if ((rc = pipe.begin(pops, n_pops, A, n_steps, s))) return rc;
+  // PhasePrecessingPlaceCells: each population's clock of step st, t_st = t_{st-1} + dt like Agent.update's
+  std::vector<double> t_pop((size_t)n_pops, 0.0);
+  for (int p = 0; p < n_pops; ++p)
+    if (pops[p].kind == RIAB_CELLS_PPPC && pops[p].cells != nullptr) t_pop[p] = ((const riab_pppc_cells*)pops[p].cells)->t;
   for (int64_t st = 0; st < n_steps; ++st) {
     if (pipe.pipe) pipe.pipe->step = st;
     const riab_step_io sio = step_io(st);
@@ -2538,7 +2630,13 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
       nz.step = pp.noise.step + (uint64_t)st; nz.dt = prm->dt;
       riab_td_cells tc;                             // an FFL population uses tc.ffl only
       riab_ffl_cells& fc = tc.ffl;
+      riab_pppc_cells ppc;
       const void* cells = pp.cells;
+      if (pp.kind == RIAB_CELLS_PPPC && pp.cells != nullptr) {
+        ppc = *(const riab_pppc_cells*)pp.cells;
+        ppc.t = t_pop[p];                           // the skewed launch evaluating step st's rates uses step st's phase
+        cells = &ppc;
+      }
       if (ffl_like(pp.kind)) {
         // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
         // previous step's: before the first step, the row the caller passed
@@ -2577,6 +2675,7 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
       else rc = launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s);
       if (rc) return rc;
     }
+    for (int p = 0; p < n_pops; ++p) t_pop[p] = t_pop[p] + prm->dt;
   }
   return 0;
 }
@@ -2998,6 +3097,13 @@ int riab_avc_rates(const double* pos_dev, int64_t n_pos, const double* other_pos
   c.n_other = other_per_position ? n_pos : 1;
   c.partner_is_self = 0;
   return rates_at(RIAB_CELLS_AVC, &c, pos_dev, n_pos, env, head_direction_dev, nullptr, nullptr, out_dev, ld_out, stream);
+}
+
+// ------------------------------------------------------ PhasePrecessingPlaceCells
+int riab_pppc_rates(const double* pos_dev, const double* velocity_dev, int64_t n_pos, const riab_env* env,
+                    const riab_pppc_cells* cells, float* out_dev, int64_t ld_out, void* stream) {
+  if (n_pos > 0 && velocity_dev == nullptr) return fail(RIAB_ERR_INVALID, "riab_pppc_rates: velocity_dev NULL");
+  return rates_at(RIAB_CELLS_PPPC, cells, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream, velocity_dev);
 }
 
 // ------------------------------------------------------------ ObjectVectorCells
