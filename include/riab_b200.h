@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define RIAB_ABI_VERSION 2
+#define RIAB_ABI_VERSION 3
 
 typedef enum {
   RIAB_OK = 0,
@@ -561,7 +561,8 @@ int riab_run_src(const riab_agents* agents, const riab_env* env, const riab_moti
  * explicit edges np.arange(extent[0], extent[1] + dx, dx) (right-most edge inclusive, outside samples dropped) --
  * and sum[(ix, iy), c] = the sum of cell c's rates over those samples.  rate map = sum / max(count, 1), laid out
  * `.T[::-1, :]` by the host like the reference (Neurons.py:483-490 plot_rate_map(method="history"),
- * Agent.py:956 plot_position_heatmap). */
+ * Agent.py:956 plot_position_heatmap).  Counts are exact 64-bit integers and sums float64 (device atomics, so the
+ * sums' last bits depend on the order the samples arrive in: about n * 2^-53 relative for n samples in a bin). */
 typedef struct {
   const float* agent_ring;     /* (agent_ring_rows, A, 8) f32 history rows (pos.xy first), riab_agent_history.ring */
   int32_t agent_ring_rows;
@@ -574,8 +575,8 @@ typedef struct {
   int32_t reserved;
 } riab_history_view;
 int riab_history_rate_maps(const riab_history_view* h, const double* edges_x_dev, int32_t n_edges_x,
-                           const double* edges_y_dev, int32_t n_edges_y, float* sum_dev /* ((nx*ny), ld), zeroed here */,
-                           float* count_dev /* (nx*ny), zeroed here */, void* stream);
+                           const double* edges_y_dev, int32_t n_edges_y, double* sum_dev /* ((nx*ny), ld), zeroed here */,
+                           uint64_t* count_dev /* (nx*ny), zeroed here */, void* stream);
 
 /* Number of kernels launched by the library since load (bench.py "gpu_launches"). */
 int64_t riab_launch_count(void);

@@ -754,7 +754,7 @@ class Agent:
         if neurons is not None:
             n = min(n, min(neurons._hist_rows, neurons._hist_cap) if neurons._hist is not None else 0)
         nx, ny = len(ex) - 1, len(ey) - 1
-        count = torch.zeros(nx * ny, dtype=torch.float32, device=self.device)
+        count = torch.zeros(nx * ny, dtype=torch.int64, device=self.device)
         ssum = None
         if n > 0:
             h = _lib.HistoryView()
@@ -762,7 +762,7 @@ class Agent:
             h.agent_row0 = int((self._hist_rows - n) % self._hist_cap)
             h.n_steps, h.n_agents = n, self.n_agents
             if neurons is not None:
-                ssum = torch.zeros((nx * ny, neurons._ld()), dtype=torch.float32, device=self.device)
+                ssum = torch.zeros((nx * ny, neurons._ld()), dtype=torch.float64, device=self.device)
                 h.rates_ring, h.rates_ring_rows = neurons._hist.data_ptr(), int(neurons._hist_cap)
                 h.rates_row0 = int((neurons._hist_rows - n) % neurons._hist_cap)
                 h.ld, h.n_cells = neurons._ld(), neurons.n
@@ -771,9 +771,9 @@ class Agent:
             _lib.check(self._lib.riab_history_rate_maps(C.byref(h), exd.data_ptr(), len(ex), eyd.data_ptr(), len(ey),
                                                         ssum.data_ptr() if ssum is not None else None, count.data_ptr(),
                                                         self._stream()))
-        count = count.cpu().numpy().astype(np.float64).reshape(nx, ny)
+        count = count.cpu().numpy().astype(np.float64).reshape(nx, ny)          # exact: counts stay below 2^53
         if ssum is not None:
-            ssum = ssum.cpu().numpy().astype(np.float64)[:, : neurons.n].reshape(nx, ny, neurons.n)
+            ssum = ssum[:, : neurons.n].cpu().numpy().reshape(nx, ny, neurons.n)
         elif neurons is not None:
             ssum = np.zeros((nx, ny, neurons.n))
         return count, ssum

@@ -177,6 +177,7 @@ SYMBOLS = {
     "riab_last_error": (C.c_char_p, []),
     "riab_launch_count": (C.c_int64, []),
     "riab_stream_synchronize": (C.c_int, [C.c_void_p]),
+    # (view, edges_x f64, n, edges_y f64, n, sum f64 or NULL, count u64, stream): device pointers
     "riab_history_rate_maps": (C.c_int, [C.POINTER(HistoryView), C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "riab_agent_update": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO), C.c_void_p]),
@@ -272,7 +273,7 @@ def load():
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)      # AttributeError if the symbol is not exported
         fn.restype, fn.argtypes = res, args
-    if lib.riab_abi_version() != 2:
+    if lib.riab_abi_version() != 3:
         raise ImportError("libriab_b200.so ABI version mismatch")
     _lib = lib
     return lib

@@ -1518,7 +1518,9 @@ __global__ void __launch_bounds__(NT) k_bvc_integrate_ego(const BvcConst bc, con
 // ---------------------------------------------------------------------------
 // History analytics: occupancy and rate-weighted histograms of the agents' positions (utils.py:544-589).
 // np.histogram2d with explicit edges: bin = searchsorted(edges, x, 'right') - 1, the right-most edge belongs to
-// the last bin, samples outside are dropped.
+// the last bin, samples outside are dropped.  Counts are 64-bit integers and rate sums float64: a default Agent ring of
+// 65 536 agents holds 2^26 samples, a float32 count stops at 2^24 and a float32 running sum of millions of rates drifts
+// by about 1e-2 relative, while any order of a float64 sum of n float32 rates agrees to about n * 2^-53 relative.
 __device__ __forceinline__ int hist_bin(const double* __restrict__ e, int n_edges, double x) {
   if (!(x >= e[0]) || !(x <= e[n_edges - 1])) return -1;
   if (x == e[n_edges - 1]) return n_edges - 2;
@@ -1530,8 +1532,8 @@ __device__ __forceinline__ int hist_bin(const double* __restrict__ e, int n_edge
   return lo - 1;
 }
 __global__ void __launch_bounds__(NT) k_history_maps(const riab_history_view h, const double* __restrict__ ex, int nex,
-                                                     const double* __restrict__ ey, int ney, float* __restrict__ sum,
-                                                     float* __restrict__ count) {
+                                                     const double* __restrict__ ey, int ney, double* __restrict__ sum,
+                                                     unsigned long long* __restrict__ count) {
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (NT / 32);
   const long long n_samples = h.n_steps * h.n_agents;
@@ -1543,12 +1545,12 @@ __global__ void __launch_bounds__(NT) k_history_maps(const riab_history_view h, 
     const int ix = hist_bin(ex, nex, (double)p[0]), iy = hist_bin(ey, ney, (double)p[1]);
     if (ix < 0 || iy < 0) continue;                              // warp-uniform
     const long long bin = (long long)ix * ny + iy;
-    if (lane == 0) atomicAdd(count + bin, 1.0f);
+    if (lane == 0) atomicAdd(count + bin, 1ull);
     if (h.rates_ring != nullptr) {
       const long long rrow = (h.rates_row0 + step) % h.rates_ring_rows;
       const float* r = h.rates_ring + (rrow * h.n_agents + agent) * h.ld;
-      float* dst = sum + bin * h.ld;
-      for (int c = lane; c < h.n_cells; c += 32) atomicAdd(dst + c, r[c]);
+      double* dst = sum + bin * h.ld;
+      for (int c = lane; c < h.n_cells; c += 32) atomicAdd(dst + c, (double)r[c]);
     }
   }
 }
@@ -2709,7 +2711,7 @@ extern "C" {
 int riab_abi_version(void) { return RIAB_ABI_VERSION; }
 const char* riab_last_error(void) { return g_err; }
 int riab_history_rate_maps(const riab_history_view* h, const double* edges_x_dev, int32_t n_edges_x,
-                           const double* edges_y_dev, int32_t n_edges_y, float* sum_dev, float* count_dev, void* stream) {
+                           const double* edges_y_dev, int32_t n_edges_y, double* sum_dev, uint64_t* count_dev, void* stream) {
   if (h == nullptr || h->agent_ring == nullptr || edges_x_dev == nullptr || edges_y_dev == nullptr || count_dev == nullptr)
     return fail(RIAB_ERR_INVALID, "riab_history_rate_maps: NULL argument");
   if (n_edges_x < 2 || n_edges_y < 2 || h->agent_ring_rows <= 0 || h->n_steps < 0 || h->n_agents <= 0)
@@ -2718,8 +2720,8 @@ int riab_history_rate_maps(const riab_history_view* h, const double* edges_x_dev
     return fail(RIAB_ERR_INVALID, "riab_history_rate_maps: rates ring without sum_dev / ld < n_cells");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t bins = (size_t)(n_edges_x - 1) * (size_t)(n_edges_y - 1);
-  RIAB_CUDA_OK(cudaMemsetAsync(count_dev, 0, bins * sizeof(float), s));
-  if (h->rates_ring != nullptr) RIAB_CUDA_OK(cudaMemsetAsync(sum_dev, 0, bins * (size_t)h->ld * sizeof(float), s));
+  RIAB_CUDA_OK(cudaMemsetAsync(count_dev, 0, bins * sizeof(uint64_t), s));
+  if (h->rates_ring != nullptr) RIAB_CUDA_OK(cudaMemsetAsync(sum_dev, 0, bins * (size_t)h->ld * sizeof(double), s));
   const long long n_samples = h->n_steps * h->n_agents;
   if (n_samples == 0) return 0;
   int dev = 0, sms = 0;
@@ -2727,7 +2729,8 @@ int riab_history_rate_maps(const riab_history_view* h, const double* edges_x_dev
   RIAB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   long long blocks = (n_samples + NT / 32 - 1) / (NT / 32);
   if (blocks > sms * 8ll) blocks = sms * 8ll;
-  k_history_maps<<<(unsigned)blocks, NT, 0, s>>>(*h, edges_x_dev, n_edges_x, edges_y_dev, n_edges_y, sum_dev, count_dev);
+  k_history_maps<<<(unsigned)blocks, NT, 0, s>>>(*h, edges_x_dev, n_edges_x, edges_y_dev, n_edges_y, sum_dev,
+                                                 (unsigned long long*)count_dev);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in riab_b200.h but not exported"
         assert name in _lib.SYMBOLS, f"{name} has no ctypes prototype"
-    assert lib.riab_abi_version() == 2
+    assert lib.riab_abi_version() == 3
     assert lib.riab_launch_count() == 0
 
 

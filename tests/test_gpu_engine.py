@@ -347,7 +347,7 @@ def test_zero_copy_host_io_equals_staged_copies():
 def test_history_rate_maps_on_the_device():
     """riab_history_rate_maps: occupancy and rate maps binned from the device history rings equal
     utils.bin_data_for_histogramming (utils.py:544-589) applied to the same history on the host -- counts exactly
-    (same np.histogram2d edge semantics), rate sums to float32 atomics' accuracy."""
+    (same np.histogram2d edge semantics), rate sums to float32 accuracy (test_gpu_history_maps.py bounds them by float64 sums)."""
     import ratinabox_b200 as rb
     A, steps = 300, 40
     E, Ag = make(rb, A, dt=0.05)

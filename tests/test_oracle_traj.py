@@ -164,7 +164,7 @@ def test_structs_have_the_headers_layout(tmp_path):
     got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
     assert got == [C.sizeof(_lib.Trajectory), _lib.Trajectory.t_max.offset, C.sizeof(_lib.MotionSource),
                    _lib.MotionSource.t.offset, _lib.MotionSource.traj.offset, _lib.MotionSource.forced_dev.offset,
-                   _lib.MOTION_RANDOM, _lib.MOTION_IMPORTED, _lib.MOTION_FORCED, 2]
+                   _lib.MOTION_RANDOM, _lib.MOTION_IMPORTED, _lib.MOTION_FORCED, 3]
 
 
 def test_trajectory_kernels_do_not_spill():
