@@ -168,6 +168,53 @@ typedef struct {
 int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
                           const riab_step_io* io, const riab_motion_source* src, void* stream);
 
+/* ------------------------------------------------------ ThetaSequenceAgent
+ * contribs/SubAgent.py:182-356: the position of a theta sweep over a lead Agent's batch at one lead step, written to
+ * out_pos; the ThetaSequenceAgent then moves there with riab_agent_update_src (RIAB_MOTION_FORCED).  The host computes
+ * the theta phase from the lead's clock (:266-267), so `phase` is the same for every agent:
+ *   RIAB_THETA_NONE        before the look-behind or after the look-ahead (:270-271, :337-338): NaN
+ *   RIAB_THETA_BEHIND      :274-300: interp1d over rows [idx-3, idx+3) of the window of the lead's recent rows, idx the
+ *                          first arg-min of |distance - target|; the lead's position while its distance is < d_half.
+ *                          Where the reference raises (idx < 3, or target outside those rows) the two window rows that
+ *                          bracket the target are interpolated; a target before the window gives NaN.
+ *   RIAB_THETA_AHEAD_FIRST :305-327: the forward agent starts from the lead's pos / velocity / rotational velocity /
+ *                          distance (its measured velocity and head direction carry over); stop = distance + forward_distance
+ *   RIAB_THETA_AHEAD       :328-334: the forward agent advances (at least one step per rollout) while its distance is
+ *                          below both the query and the stop; the position interpolates its last two samples.  A query
+ *                          past the stop or behind the kept pair gives NaN.
+ * target / query = lead distance + offset (-distance_back / +distance_ahead, host float64).  Any position farther than
+ * d_half from the lead's (periodic boundaries wrap) becomes NaN (:341-343).  The lead's (x, y, distance) row is appended
+ * to the ring at ring_head on every call (:259-264). */
+typedef enum { RIAB_THETA_NONE = 0, RIAB_THETA_BEHIND = 1, RIAB_THETA_AHEAD_FIRST = 2, RIAB_THETA_AHEAD = 3 } riab_theta_phase;
+typedef struct {
+  int64_t n_agents;
+  int64_t id_offset;                      /* global id of row 0 (keys the forward rollouts' Philox stream) */
+  const double* lead_pos;                 /* (A,2) device: the lead Agent's state after its update */
+  const double* lead_velocity;            /* (A,2) */
+  const double* lead_rotational_velocity; /* (A) */
+  const double* lead_distance;            /* (A) distance_travelled */
+  double* ring;                           /* (3, ring_rows, A) f64: lead x, y, distance of the recent lead steps */
+  int64_t ring_rows;
+  int64_t ring_head;                      /* slot of this step's row */
+  int64_t window;                         /* 1 <= window <= ring_rows rows end at ring_head (RIAB_THETA_BEHIND) */
+  riab_agents fwd;                        /* forward agent state (id_offset ignored) */
+  double* fwd_pair;                       /* (A,3) distance, x, y of the forward agent's previous rollout sample */
+  double* fwd_stop;                       /* (A) stop distance of the current rollout */
+  int64_t* fwd_steps;                     /* (A) rollout steps taken */
+  const double* xi_forward;               /* (A, xi_steps, 2) injected standard normals of rollout steps 0.. or NULL; */
+  int64_t xi_steps;                       /*   steps >= xi_steps draw Philox4x32-10(seed, rollout, step, agent id) */
+  uint64_t seed;
+  uint64_t rollout;                       /* rollout counter (Philox sub-index) */
+  int32_t phase;                          /* riab_theta_phase */
+  int32_t reserved;
+  double d_half;
+  double offset;
+  double forward_distance;                /* d_half + 100 average_measured_speed (theta_frac / 2) T_theta */
+  double* out_pos;                        /* (A,2) device */
+} riab_theta_seq;
+/* fwd_prm: the forward agent's motion parameters, dt = lead dt * v_sequence / average_measured_speed. */
+int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const riab_motion_params* fwd_prm, void* stream);
+
 /* ----------------------------------------------------------------- PlaceCells */
 typedef enum { RIAB_PC_GAUSSIAN = 0, RIAB_PC_GAUSSIAN_THRESHOLD = 1, RIAB_PC_DIFF_OF_GAUSSIANS = 2,
                RIAB_PC_TOP_HAT = 3, RIAB_PC_ONE_HOT = 4 } riab_pc_description;   /* Neurons.py:959-976 */

@@ -486,8 +486,8 @@ class Agent:
         if not self.fused_step and not self._staging_only:
             self._flush_pending()                      # launch the motion kernel now (asynchronous)
 
-    def _fill_motion_params(self, dt, kwargs, drift_to_random_strength_ratio=1):
-        mp = self._mp
+    def _fill_motion_params(self, dt, kwargs, drift_to_random_strength_ratio=1, mp=None):
+        mp = self._mp if mp is None else mp
         mp.dt = float(dt)
         mp.speed_coherence_time_kw = float(kwargs.get("speed_coherence_time", self.speed_coherence_time))
         mp.speed_mean_kw = float(kwargs.get("speed_mean", self.speed_mean))

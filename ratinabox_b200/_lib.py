@@ -56,6 +56,19 @@ class MotionSource(C.Structure):
 MOTION_RANDOM, MOTION_IMPORTED, MOTION_FORCED = 0, 1, 2      # riab_motion_kind
 
 
+class ThetaSeq(C.Structure):
+    _fields_ = [("n_agents", C.c_int64), ("id_offset", C.c_int64), ("lead_pos", C.c_void_p), ("lead_velocity", C.c_void_p),
+                ("lead_rotational_velocity", C.c_void_p), ("lead_distance", C.c_void_p), ("ring", C.c_void_p),
+                ("ring_rows", C.c_int64), ("ring_head", C.c_int64), ("window", C.c_int64), ("fwd", Agents),
+                ("fwd_pair", C.c_void_p), ("fwd_stop", C.c_void_p), ("fwd_steps", C.c_void_p), ("xi_forward", C.c_void_p),
+                ("xi_steps", C.c_int64), ("seed", C.c_uint64), ("rollout", C.c_uint64), ("phase", C.c_int32),
+                ("reserved", C.c_int32), ("d_half", C.c_double), ("offset", C.c_double), ("forward_distance", C.c_double),
+                ("out_pos", C.c_void_p)]
+
+
+THETA_NONE, THETA_BEHIND, THETA_AHEAD_FIRST, THETA_AHEAD = 0, 1, 2, 3   # riab_theta_phase
+
+
 class PlaceCells(C.Structure):
     _fields_ = [("n_cells", C.c_int32), ("description", C.c_int32), ("wall_geometry", C.c_int32),
                 ("n_inner_walls", C.c_int32), ("min_fr", C.c_float), ("max_fr", C.c_float),
@@ -184,6 +197,7 @@ SYMBOLS = {
     "riab_trajectory_build": (C.c_int, [C.POINTER(Trajectory), c_double_p, C.c_void_p]),
     "riab_agent_update_src": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                         C.POINTER(MotionSource), C.c_void_p]),
+    "riab_theta_seq_step": (C.c_int, [C.POINTER(ThetaSeq), C.POINTER(Env), C.POINTER(MotionParams), C.c_void_p]),
     "riab_place_pack_floats": (C.c_int64, [C.c_int32, C.c_int32]),
     "riab_place_pack": (C.c_int, [c_double_p, c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_int32, c_double_p,
                                   C.c_int32, C.POINTER(PlaceCells), c_float_p]),

@@ -12,6 +12,7 @@
 //   k_bvc_rays<TABLE>   BVC phase A (float64 rays)
 //   k_bvc_integrate     BVC phase B (float32 angular integral, TMA-staged tables)
 //   k_td_*              TD learning of ValueNeuron / SuccessorFeatures (riab_td.cuh)
+//   k_theta_seq         ThetaSequenceAgent sweep positions over a lead Agent's batch, one agent per thread (float64)
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -34,6 +35,7 @@
 #include "riab_rsn.cuh"
 #include "riab_traj.cuh"
 #include "riab_td.cuh"
+#include "riab_theta.cuh"
 
 using namespace riab;
 
@@ -2798,6 +2800,119 @@ int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const 
   MotionDerived md;
   derive_motion(*prm, md);
   k_agent_update_src<<<(unsigned)((agents->n_agents + 127) / 128), 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, sk, ek);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------- ThetaSequenceAgent
+// One agent per thread: append the lead's row to the look-behind ring, then the sweep position of this step
+// (riab_theta.cuh).  Look-ahead steps advance the agent's forward rollout with motion_step in place.
+__global__ void __launch_bounds__(128) k_theta_seq(const riab_theta_seq ts, const riab_motion_params mp,
+                                                   const MotionDerived md, const EnvK env) {
+  __shared__ __align__(16) double s_walls[MAXW * 4];
+  __shared__ uint64_t s_bar;
+  stage_walls(s_walls, &s_bar, env);
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ts.n_agents) return;
+  const long long A = ts.n_agents, R = ts.ring_rows;
+  const double2 lp = reinterpret_cast<const double2*>(ts.lead_pos)[i];
+  const double ld = ts.lead_distance[i];
+  const long long row = ts.ring_head * A + i;
+  ts.ring[row] = lp.x;
+  ts.ring[R * A + row] = lp.y;
+  ts.ring[2 * R * A + row] = ld;
+
+  double px = theta_nan(), py = theta_nan();
+  const double target = __dadd_rn(ld, ts.offset);
+  if (ts.phase == RIAB_THETA_BEHIND) {
+    if (ld < ts.d_half) {
+      px = lp.x; py = lp.y;
+    } else {
+      ThetaWindow W;
+      W.ring = ts.ring; W.A = A; W.R = R; W.w = ts.window; W.i = i;
+      W.first = ts.ring_head - (ts.window - 1);
+      if (W.first < 0) W.first += R;
+      theta_look_behind(W, target, px, py);
+    }
+  } else if (ts.phase == RIAB_THETA_AHEAD_FIRST || ts.phase == RIAB_THETA_AHEAD) {
+    AgentState s;
+    load_agent(ts.fwd, i, s);
+    double2 prev;
+    double d_prev;
+    long long k;
+    double stop;
+    if (ts.phase == RIAB_THETA_AHEAD_FIRST) {
+      const double2 lv = reinterpret_cast<const double2*>(ts.lead_velocity)[i];
+      s.px = lp.x; s.py = lp.y; s.vx = lv.x; s.vy = lv.y;
+      s.rot = ts.lead_rotational_velocity[i];
+      s.dist = ld;
+      k = 0;
+      stop = __dadd_rn(ld, ts.forward_distance);
+      ts.fwd_stop[i] = stop;
+      d_prev = s.dist; prev = make_double2(s.px, s.py);
+    } else {
+      k = ts.fwd_steps[i];
+      stop = ts.fwd_stop[i];
+      d_prev = ts.fwd_pair[3 * i]; prev = make_double2(ts.fwd_pair[3 * i + 1], ts.fwd_pair[3 * i + 2]);
+    }
+    const unsigned long long gid = (unsigned long long)(ts.id_offset + i);
+    const double f1 = __longlong_as_double((long long)ts.seed);
+    while (k == 0 || (s.dist < target && s.dist < stop)) {
+      d_prev = s.dist; prev = make_double2(s.px, s.py);
+      double n1, n2;
+      if (ts.xi_forward != nullptr && k < ts.xi_steps) {
+        n1 = ts.xi_forward[2 * (i * ts.xi_steps + k)];
+        n2 = ts.xi_forward[2 * (i * ts.xi_steps + k) + 1];
+      } else {
+        theta_fwd_normals(ts.seed, ts.rollout, (unsigned long long)k, gid, n1, n2);
+      }
+      // exactly-zero displacement / polygon re-draw fall-backs: keyed by rollout, step and agent
+      const double f2 = __longlong_as_double((long long)(((unsigned long long)k | (ts.rollout << 32)) ^ (gid << 20) ^
+                                                         0x5448455441000000ull));
+      motion_step<false>(s, s_walls, env.W, mp, md, env.ext, env.periodic != 0, env.scale, env.polygon != 0, env.nb, env.h0,
+                         env.nh, n1, n2, false, 0.0, 0.0, f1, f2, nullptr, nullptr, nullptr);
+      ++k;
+    }
+    store_agent(ts.fwd, i, s);
+    ts.fwd_steps[i] = k;
+    ts.fwd_pair[3 * i] = d_prev; ts.fwd_pair[3 * i + 1] = prev.x; ts.fwd_pair[3 * i + 2] = prev.y;
+    if (s.dist >= target && target >= d_prev) {
+      px = interp_linear(target, d_prev, s.dist, prev.x, s.px);
+      py = interp_linear(target, d_prev, s.dist, prev.y, s.py);
+    }
+  }
+  // SubAgent.py:341-343: farther than d_half from the lead (a sweep interpolated across a periodic boundary) -> NaN
+  if (px == px && py == py) {
+    D vx, vy;
+    step_displacement(D(px), D(py), D(lp.x), D(lp.y), env.periodic != 0, env.scale, vx, vy);
+    if (dsqrt(vx * vx + vy * vy).v > ts.d_half) px = py = theta_nan();
+  }
+  reinterpret_cast<double2*>(ts.out_pos)[i] = make_double2(px, py);
+}
+
+int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const riab_motion_params* fwd_prm, void* stream) {
+  EnvK ek;
+  int rc;
+  if (ts == nullptr) return fail(RIAB_ERR_INVALID, "riab_theta_seq_step: ts is NULL");
+  if ((rc = make_env(env, ek)) || (rc = check_motion(fwd_prm))) return rc;
+  if (ts->phase < RIAB_THETA_NONE || ts->phase > RIAB_THETA_AHEAD) return fail(RIAB_ERR_INVALID, "bad theta phase %d", ts->phase);
+  if (ts->n_agents < 0) return fail(RIAB_ERR_INVALID, "n_agents < 0");
+  if (ts->n_agents == 0) return 0;
+  if (!ts->lead_pos || !ts->lead_velocity || !ts->lead_rotational_velocity || !ts->lead_distance || !ts->ring ||
+      !ts->fwd_pair || !ts->fwd_stop || !ts->fwd_steps || !ts->out_pos)
+    return fail(RIAB_ERR_INVALID, "riab_theta_seq_step: NULL array");
+  riab_agents fwd = ts->fwd;
+  fwd.n_agents = ts->n_agents;
+  if ((rc = check_agents(&fwd))) return rc;
+  if (ts->ring_rows < 1 || ts->ring_head < 0 || ts->ring_head >= ts->ring_rows)
+    return fail(RIAB_ERR_INVALID, "ring_head %lld outside a ring of %lld rows", (long long)ts->ring_head, (long long)ts->ring_rows);
+  if (ts->phase == RIAB_THETA_BEHIND && (ts->window < 1 || ts->window > ts->ring_rows))
+    return fail(RIAB_ERR_INVALID, "window %lld outside [1, ring_rows = %lld]", (long long)ts->window, (long long)ts->ring_rows);
+  if (ts->xi_forward != nullptr && ts->xi_steps < 0) return fail(RIAB_ERR_INVALID, "xi_steps < 0");
+  MotionDerived md;
+  derive_motion(*fwd_prm, md);
+  k_theta_seq<<<(unsigned)((ts->n_agents + 127) / 128), 128, 0, (cudaStream_t)stream>>>(*ts, *fwd_prm, md, ek);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;

@@ -74,7 +74,8 @@ RIAB_DEV void philox_round_keys(uint32_t (&rk)[2 * R], unsigned long long seed) 
 
 // Stream ids (third counter word, top byte)
 enum : uint32_t { RIAB_STREAM_AGENT_OU = 0, RIAB_STREAM_CELL_NOISE = 1, RIAB_STREAM_SPIKES = 2, RIAB_STREAM_MEASURE = 3,
-                  RIAB_STREAM_THIN = 4 };          // thinned spikes: calls n = 0, 1, ... of a (row, 128-cell block), n in bits 16.. of the sub-index
+                  RIAB_STREAM_THIN = 4,            // thinned spikes: calls n = 0, 1, ... of a (row, 128-cell block), n in bits 16.. of the sub-index
+                  RIAB_STREAM_THETA_FWD = 5 };     // ThetaSequenceAgent forward rollouts: sub-index = rollout, step = rollout step
 
 // counter = (agent id lo32, sub-index, step lo32, (step hi & 0xffff) | stream<<24 | population<<16)
 RIAB_HD void philox_ctr(uint32_t (&c)[4], uint64_t agent, uint32_t sub, uint64_t step, uint32_t stream, uint32_t pop) {
@@ -91,13 +92,11 @@ RIAB_HD double u01_53(uint32_t hi, uint32_t lo) {
 }
 RIAB_HD float u01_24(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 
-// Two standard normals for the agent OU draws: Philox4x32-10 -> two 32-bit uniforms ->
+// Two standard normals of the Philox counter c (the agent OU draws): Philox4x32-10 -> two 32-bit uniforms ->
 // Box-Muller in float32 (logf / sqrtf / sincospif are the accurate single-precision routines),
 // widened to double.  The draws are noise: their float32 resolution is irrelevant to the
 // dynamics, and float32 keeps ~150 dependent float64 operations off the motion chain.
-RIAB_DEV void agent_normals(uint64_t seed, uint64_t step, uint64_t agent, double& n1, double& n2) {
-  uint32_t c[4];
-  philox_ctr(c, agent, 0u, step, RIAB_STREAM_AGENT_OU, 0u);
+RIAB_DEV void philox_normals(uint32_t (&c)[4], uint64_t seed, double& n1, double& n2) {
   philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
   const float u1 = fmaf(__uint2float_rn(c[0]), 2.3283064365386963e-10f, 1.1641532182693481e-10f);   // (0,1]
   const float u2 = __uint2float_rn(c[2]) * 2.3283064365386963e-10f;                                  // [0,1]
@@ -105,6 +104,11 @@ RIAB_DEV void agent_normals(uint64_t seed, uint64_t step, uint64_t agent, double
   float s, co;
   sincospif(2.0f * u2, &s, &co);
   n1 = (double)(r * co); n2 = (double)(r * s);
+}
+RIAB_DEV void agent_normals(uint64_t seed, uint64_t step, uint64_t agent, double& n1, double& n2) {
+  uint32_t c[4];
+  philox_ctr(c, agent, 0u, step, RIAB_STREAM_AGENT_OU, 0u);
+  philox_normals(c, seed, n1, n2);
 }
 
 // ---------------------------------------------------------------------------
