@@ -260,6 +260,8 @@ typedef struct {
   float min_fr, max_fr;
   const float* packed_dev; /* riab_grid_pack output */
   int32_t n_pad;           /* filled by riab_grid_pack */
+  int32_t phase_turns;     /* filled by riab_grid_pack: 1 = the block holds wave vectors and phases in turns, for the
+                              compensated phase of large |k| r_max (riab_grid.cuh); 0 = radians */
 } riab_grid_cells;
 int64_t riab_grid_pack_floats(int32_t n_cells);
 int riab_grid_pack(const double* gridscales_host, const double* phase_offsets_host /* (N,2) */,

@@ -79,7 +79,8 @@ class PlaceCells(C.Structure):
 
 class GridCells(C.Structure):
     _fields_ = [("n_cells", C.c_int32), ("description", C.c_int32), ("width_ratio", C.c_double),
-                ("min_fr", C.c_float), ("max_fr", C.c_float), ("packed_dev", C.c_void_p), ("n_pad", C.c_int32)]
+                ("min_fr", C.c_float), ("max_fr", C.c_float), ("packed_dev", C.c_void_p), ("n_pad", C.c_int32),
+                ("phase_turns", C.c_int32)]
 
 
 class BvcCells(C.Structure):

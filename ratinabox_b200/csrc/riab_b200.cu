@@ -358,12 +358,14 @@ __device__ __forceinline__ void finish4(float (&o)[4], const OutK& out, const Ta
 
 // ---------------------------------------------------------------------------
 // Cell-type policies for the step kernel.
-template <int WI, int DESC>
+// COMP: the compensated direct form (PlaceConst::comp, riab_place.cuh): kernels of their own, chosen by the host, so the
+// expanded and geodesic kernels keep their code and registers.
+template <int WI, int DESC, bool COMP = false>
 struct PlacePolicy {
   using Const = PlaceConst;
   using Regs = PlaceCellRegs<WI>;
   static constexpr int REC = place_rec(WI);
-  static constexpr bool LIGHT = (WI == 0) && (DESC >= 0);   // few instructions per rate: HBM-bound consumers
+  static constexpr bool LIGHT = (WI == 0) && (DESC >= 0) && !COMP;   // few instructions per rate: HBM-bound consumers
   // rates lie in [min_fr, max_fr], so the thinned spike stream applies, but it measured slower for place cells: the
   // Euclidean Gaussian loop is HBM-bound and hides the dense stream's instructions under its stores, the line-of-sight
   // loop with the post-pass needs 8 producer warps and loses next to them.  The dense stream stays.
@@ -375,19 +377,24 @@ struct PlacePolicy {
   }
   static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double, double, double, double, double, double,
                                                 const double* s_walls, const double* aux, const Const& c, const EnvK& env) {
-    place_agent_record<WI>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
+    place_agent_record<WI, COMP>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
   }
-  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI>(r, c, cell0); }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI, COMP>(r, c, cell0); }
   template <bool DEFER, int EXP = -1>
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int cell0,
                                                 const float* rec, uint32_t inner_s, bool& unsure) {
-    place_rates4<WI, DESC, DEFER, EXP>(o, r, c, cell0, rec, inner_s, unsure);
+    place_rates4<WI, DESC, DEFER, EXP, COMP>(o, r, c, cell0, rec, inner_s, unsure);
   }
   // 0: direct form, 1: expanded exponent, 2: expanded with the [0, max_fr] scale folded into the exponent
-  static __device__ __forceinline__ int expanded(const Const& c) { return (DESC == RIAB_PC_GAUSSIAN && c.expanded) ? 1 + c.fold : 0; }
+  static __device__ __forceinline__ int expanded(const Const& c) {
+    return (!COMP && DESC == RIAB_PC_GAUSSIAN && c.expanded) ? 1 + c.fold : 0;
+  }
   static __device__ __forceinline__ int wall0(const Const& c) { return c.wall0; }
 };
 
+// TURNS = 1: the block holds turns (riab_grid_cells::phase_turns) and the rates take the compensated phase.  A kernel of
+// its own, chosen by the host: the radian kernels keep their code and registers.
+template <int TURNS>
 struct GridPolicy {
   using Const = GridConst;
   using Regs = GridCellRegs;
@@ -406,7 +413,7 @@ struct GridPolicy {
   template <bool DEFER, int EXP = -1>
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
                                                 uint32_t, bool&) {
-    grid_rates4(o, r, c, rec);
+    grid_rates4<TURNS>(o, r, c, rec);
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const&) { return 0; }
@@ -499,9 +506,9 @@ struct AvcPolicy {
 // PhasePrecessingPlaceCells: PlacePolicy's record, cells and rates (direct exponent form), times the theta modulation
 // factor of riab_pppc.cuh.  MODE 0 reads the rows' velocities from Const::vel (given_dir: the one given vector stands for
 // every kinematic input).
-template <int WI, int DESC>
+template <int WI, int DESC, bool COMP = false>
 struct PppcPolicy {
-  using Place = PlacePolicy<WI, DESC>;
+  using Place = PlacePolicy<WI, DESC, COMP>;
   using Const = PppcConst;
   using Regs = PppcCellRegs<WI>;
   static constexpr int REC = pppc_rec(WI);
@@ -1189,8 +1196,14 @@ __global__ void __launch_bounds__(NT) k_place_onehot(const EnvK env, const Place
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) best = fminf(best, __shfl_xor_sync(0xffffffffu, best, o));
-  // geodesic detours are shorter than 1000: every blocked cell is a candidate there
-  const float thr = (pc.geometry == RIAB_GEOM_GEODESIC && pc.n_inner > 0) ? INFINITY : best * (1.0f + 1e-5f) + 1e-12f;
+  // Every cell whose true distance ties the true minimum passes the screen: with E a bound on |d_f - d| (the float32
+  // rounding of the centred coordinates, coord_err from make_place plus this row's |p'|), the true minimum is at most
+  // sqrt(best) + E and such a cell's float32 square at most (sqrt(best) + 2E)^2, both up to the float32 rounding of d^2.
+  // Geodesic detours are shorter than 1000: every blocked cell is a candidate there.
+  const double E = (double)pc.coord_err + 1.2e-7 * ((double)fabsf(pxf) + (double)fabsf(pyf));
+  const double sb = sqrt((double)best) * (1.0 + 1e-6) + 2.0 * E;
+  const float thr = (pc.geometry == RIAB_GEOM_GEODESIC && pc.n_inner > 0) ? INFINITY
+                    : fmaxf(best * (1.0f + 1e-5f) + 1e-12f, (float)(sb * sb * (1.0 + 1e-6)));
   double bd = INFINITY;
   int bi = 0x7fffffff;
   for (int cell = lane; cell < pc.n_cells; cell += 32) {
@@ -1687,7 +1700,24 @@ int make_place(const riab_place_cells* pc, const EnvK& env, PlaceConst& c) {
   c.kx = -pc->k_uniform;
   c.fold = (c.expanded && pc->min_fr == 0.f && c.span > 0.f) ? 1 : 0;
   c.lspan = c.fold ? log2f(c.span) : 0.f;
+  // The direct form rounds p' and c' to float32 separately, |d_f - d| ~ 2^-24 (|p'| + |c'|): a relative rate error of
+  // ~ d |d_f - d| / w^2, 2.5e-5 at 3.7 w with w = 0.05 in a 10 m box and near 1e-5 already at w = 0.05 in the unit box.
+  // Every direct-form launch without geodesic detours (which use ep0 / ep1) therefore takes the compensated kernels.
+  c.comp = (!c.expanded && pc->wall_geometry != RIAB_GEOM_GEODESIC && pc->description != RIAB_PC_ONE_HOT) ? 1 : 0;
   c.periodic = env.periodic; c.scale = env.scale; c.scale_f = (float)env.scale; c.half_f = (float)(env.scale / 2);
+  c.scale_lo = (float)(env.scale - (double)c.scale_f);
+  {
+    // Float32 error of a centre -> position distance, |d_f - d| <= 2^-23 (|p'|_1 + |c'|_1 [+ 2 scale when wrapped]):
+    // each coordinate is rounded once (2^-24 |.|), the difference once more (2^-24 |dx| <= 2^-24 (|p'x| + |c'x|)), and
+    // the wrap adds the rounding of scale and of scale - dx.  |c'|_1 <= sqrt(2 r2_max).
+    const double u = 1.1920928955078125e-07;                          // 2^-23
+    const double c1 = sqrt(2.0 * (double)pc->r2_max), per = env.periodic ? 2.0 * env.scale : 0.0;
+    c.coord_err = (float)(u * (c1 + per) * 1.001);                     // one_hot adds its row's |p'|_1 (k_place_onehot)
+    // top_hat: d^2 near w^2 is known to within 2 w E + E^2 + 2^-23 w^2, with |p'|_1 <= |c'|_1 + sqrt(2) w on the edge;
+    // pairs inside twice that band take the float64 distance (the scale-1 band 4e-6 (w^2 + 1e-3) stays the floor)
+    const double w = pc->top_hat_width, E = u * (2.0 * c1 + 1.4142135623730951 * w + per);
+    c.top_hat_band = (float)fmax(4e-6 * (w * w + 1e-3), 2.0 * (2.0 * w * E + E * E + u * w * w));
+  }
   if (env.periodic && pc->wall_geometry != RIAB_GEOM_EUCLIDEAN)
     return fail(RIAB_ERR_INVALID, "line_of_sight / geodesic wall geometry only possible when the boundary conditions are solid (Neurons.py:907-921)");
   return 0;
@@ -1709,6 +1739,7 @@ int make_grid(const riab_grid_cells* gc, const EnvK& env, GridConst& c) {
   c.As = c.A * c.span; c.Bs = fmaf(c.B, c.span, c.min_fr);
   c.clamp = c.rectify ? (c.span >= 0.f ? 1 : 2) : 0;
   c.packed = gc->packed_dev; c.cxm = env.cxm; c.cym = env.cym;
+  c.turns = gc->phase_turns ? 1 : 0;
   return 0;
 }
 
@@ -1789,6 +1820,7 @@ int make_pppc(const riab_pppc_cells* pc, const EnvK& env, const double* vel, Ppp
     return fail(RIAB_ERR_INVALID, "phase precessing place cells: theta_freq %g, sigma %g, precess_fraction %g, t %g",
                 pc->theta_freq, pc->sigma, pc->precess_fraction, pc->t);
   c.expanded = 0; c.fold = 0; c.lspan = 0.f;                          // the direct form of the DESC = -1 kernels
+  c.comp = (pc->place.wall_geometry != RIAB_GEOM_GEODESIC) ? 1 : 0;  // compensated (make_place)
   const double period = 1.0 / pc->theta_freq;
   double r = fmod(pc->t, period);                                      // Python's t % period: the sign of the divisor
   if (r != 0.0 && ((r < 0.0) != (period < 0.0))) r += period;
@@ -1879,6 +1911,13 @@ int launch_place_d(const EnvK& env, const riab_agents& ag, const riab_motion_par
                    const PlaceConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s,
                    const RunK* run = nullptr) {
   const int wi = pc.n_inner;
+  if (pc.comp) {
+    if (wi == 0) return launch_tile<PlacePolicy<0, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi == 1) return launch_tile<PlacePolicy<1, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi == 2) return launch_tile<PlacePolicy<2, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi <= 4) return launch_tile<PlacePolicy<4, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    return launch_tile<PlacePolicy<8, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  }
   if (wi == 0) return launch_tile<PlacePolicy<0, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
   if (wi == 1) return launch_tile<PlacePolicy<1, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
   if (wi == 2) return launch_tile<PlacePolicy<2, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
@@ -1921,6 +1960,13 @@ int launch_pppc(const EnvK& env, const riab_agents& ag, const riab_motion_params
                 const PppcConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s) {
   static_assert(MODE <= 2, "phase precessing place cells have no whole-run launch");
   const int wi = pc.n_inner;
+  if (pc.comp) {
+    if (wi == 0) return launch_tile<PppcPolicy<0, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+    if (wi == 1) return launch_tile<PppcPolicy<1, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+    if (wi == 2) return launch_tile<PppcPolicy<2, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+    if (wi <= 4) return launch_tile<PppcPolicy<4, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+    return launch_tile<PppcPolicy<8, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  }
   if (wi == 0) return launch_tile<PppcPolicy<0, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
   if (wi == 1) return launch_tile<PppcPolicy<1, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
   if (wi == 2) return launch_tile<PppcPolicy<2, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
@@ -2202,6 +2248,7 @@ int make_rsn(const riab_rsn_cells* r, const EnvK& env, PlaceConst& c) {
   if (r->points.wall_geometry != RIAB_GEOM_EUCLIDEAN && r->points.centres_dev == nullptr)
     return fail(RIAB_ERR_INVALID, "rsn: centres_dev NULL");
   c.expanded = 0; c.fold = 0; c.lspan = 0.f; c.kx = 0.f;
+  c.comp = 0;                          // k_rsn evaluates the plain direct form
   return 0;
 }
 
@@ -2359,7 +2406,9 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
                cudaStream_t s, BvcPipe* pipe = nullptr) {
   const double* pos_in = (MODE == 1) ? nullptr : ag.pos;
   if (d.kind == RIAB_CELLS_PLACE) return launch_place<MODE>(ek, ag, mp, io, d.place, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_GRID) return launch_tile<GridPolicy, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_GRID)
+    return d.grid.turns ? launch_tile<GridPolicy<1>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s)
+                        : launch_tile<GridPolicy<0>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, ag.n_agents, s);
@@ -2591,8 +2640,11 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
     if (pp.kind == RIAB_CELLS_PLACE)
       return src ? launch_place<4>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run)
                  : launch_place<3>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run);
-    return src ? launch_tile<GridPolicy, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
-               : launch_tile<GridPolicy, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
+    if (d.grid.turns)
+      return src ? launch_tile<GridPolicy<1>, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
+                 : launch_tile<GridPolicy<1>, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
+    return src ? launch_tile<GridPolicy<0>, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
+               : launch_tile<GridPolicy<0>, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
   }
 
   riab_motion_source src_st;                          // step st's clock: t_st = t_{st-1} + dt
@@ -2922,7 +2974,7 @@ int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const ria
 static int place_n_pad(int n) { return (n + CELL_PAD - 1) / CELL_PAD * CELL_PAD; }
 
 int64_t riab_place_pack_floats(int32_t n_cells, int32_t n_inner_walls) {
-  return (int64_t)place_n_pad(n_cells) * (4 + 2 * (n_inner_walls > 0 ? n_inner_walls : 0) + 2);
+  return (int64_t)place_n_pad(n_cells) * (4 + 2 * (n_inner_walls > 0 ? n_inner_walls : 0) + 4);
 }
 
 int riab_place_pack(const double* centres, const double* widths, int32_t n, const double* walls, int32_t n_walls,
@@ -2992,6 +3044,14 @@ int riab_place_pack(const double* centres, const double* widths, int32_t n, cons
     }
     if (j < 8) meta->eps[j] = (float)band;
   }
+  {                                                       // residuals of the centred centres (compensated direct form)
+    float* cxl = out + (size_t)(6 + 2 * n_inner) * np;
+    float* cyl = out + (size_t)(7 + 2 * n_inner) * np;
+    for (int i = 0; i < n; ++i) {
+      cxl[i] = (float)((centres[2 * i] - cxm) - (double)cx[i]);
+      cyl[i] = (float)((centres[2 * i + 1] - cym) - (double)cy[i]);
+    }
+  }
   if (geometry == RIAB_GEOM_GEODESIC && n_inner >= 1) {
     const double* w = walls + 4 * n_boundary;
     float* ce0 = out + (size_t)(4 + 2 * n_inner) * np;
@@ -3025,6 +3085,14 @@ int riab_grid_pack(const double* gridscales, const double* phase_offsets, const 
   const int np = place_n_pad(n);
   const double cxm = 0.5 * (extent[0] + extent[1]), cym = 0.5 * (extent[2] + extent[3]);
   for (int64_t i = 0; i < (int64_t)np * 9; ++i) out[i] = 0.f;
+  // The radian form rounds phases of up to |k| r_max (r_max: half-diagonal of the box) to float32 and hands them to
+  // __cosf: its rate error grows like 1.1e-7 |k| r_max of the rate scale (1.7e-6 with the default grid scales in the unit
+  // box, 1.6e-5 at scale 10).  Above |k| r_max = 40 (4.3e-6) the block holds turns for the compensated phase instead.
+  double kr = 0.0;
+  const double rmax = 0.5 * hypot(extent[1] - extent[0], extent[3] - extent[2]);
+  for (int i = 0; i < n; ++i) kr = fmax(kr, (2.0 * M_PI) / fabs(gridscales[i]) * rmax);
+  const int turns = kr > 40.0 ? 1 : 0;
+  const double unit = turns ? 1.0 / (2.0 * M_PI) : 1.0;
   for (int i = 0; i < n; ++i) {
     const double kappa = (2.0 * M_PI) / gridscales[i];
     // origin = gridscale * phase_offset / (2 pi)   (Neurons.py:1191)
@@ -3034,12 +3102,13 @@ int riab_grid_pack(const double* gridscales, const double* phase_offsets, const 
       const double wx = w[6 * i + 2 * k], wy = w[6 * i + 2 * k + 1];
       double ph = kappa * (ox * wx + oy * wy);
       ph = remainder(ph, 2.0 * M_PI);
-      out[(size_t)(3 * k + 0) * np + i] = (float)(kappa * wx);
-      out[(size_t)(3 * k + 1) * np + i] = (float)(kappa * wy);
-      out[(size_t)(3 * k + 2) * np + i] = (float)ph;
+      out[(size_t)(3 * k + 0) * np + i] = (float)(kappa * wx * unit);
+      out[(size_t)(3 * k + 1) * np + i] = (float)(kappa * wy * unit);
+      out[(size_t)(3 * k + 2) * np + i] = (float)(ph * unit);
     }
   }
   meta->n_pad = np;
+  meta->phase_turns = turns;
   return 0;
 }
 

@@ -3,7 +3,8 @@
 // (ratinabox/Environment.py:677-779) for euclidean / line_of_sight / geodesic.
 //
 // Layout of the packed per-population block (float32, written by riab_place_pack):
-//   cx[Np] | cy[Np] | k[Np] | a[Np] | per inner wall j: fc_j[Np], tc_j[Np] | ce0[Np] | ce1[Np]
+//   cx[Np] | cy[Np] | k[Np] | a[Np] | per inner wall j: fc_j[Np], tc_j[Np] | ce0[Np] | ce1[Np] | cxl[Np] | cyl[Np]
+//   cxl, cyl = the float32 residuals (c - box centre) - cx etc., read by the compensated direct form (COMP).
 //   a = -k |c|^2 (expanded Gaussian form, see place_rates4), only when all widths are equal.
 //   Np = n_cells rounded up to a multiple of 4 (padding cells sit far away, k = 0).
 //   Coordinates are relative to the box centre (halves the float32 rounding error).
@@ -73,7 +74,9 @@ RIAB_DEV void place_wall_invariants(double* __restrict__ aux, const double* __re
   }
 }
 
-template <int WI>
+// COMP: the compensated direct form -- ep0 / ep1 carry the float32 residuals of the centred position (unused slots there:
+// neither the expanded form nor geodesic detours take COMP).
+template <int WI, bool COMP = false>
 RIAB_DEV void place_agent_record(float* __restrict__ rec, double px, double py, const double* __restrict__ inner,
                                  const double* __restrict__ aux,
                                  int n_inner, int geometry, double cxm, double cym, float band, int expanded, float kx,
@@ -87,6 +90,7 @@ RIAB_DEV void place_agent_record(float* __restrict__ rec, double px, double py, 
   }
   const float pxf = (float)(px - cxm), pyf = (float)(py - cym);
   if (expanded) ep0 = (float)((double)kx * ((double)pxf * pxf + (double)pyf * pyf) + (double)lfold);   // -k |p|^2 [+ log2 span]
+  if (COMP) { ep0 = (float)((px - cxm) - (double)pxf); ep1 = (float)((py - cym) - (double)pyf); }
   *reinterpret_cast<float4*>(rec) = make_float4(pxf, pyf, ep0, ep1);
   for (int j = 0; j < WI; ++j) {
     float4 w = make_float4(-1.f, 2.f, -PLACE_QSCALE, 1.0e-6f);    // dummy wall: same side (q' < 0), X = -2, Y = 4
@@ -121,9 +125,13 @@ struct PlaceConst {                  // uniform per launch
   const float* packed;               // device
   const double* centres64;           // device (N,2)
   int periodic;                      // wrap centre->agent vectors (Environment.py:670-675)
+  int comp;                          // direct form, not geodesic: the host launches the COMP kernels (make_place)
   float scale_f, half_f;
   double scale;
   double cxm, cym;
+  float coord_err;                   // float32 error of |c' - p'| from the centres' side (make_place)
+  float top_hat_band;                // |d^2 - w^2| below which top_hat decides in float64 (make_place)
+  float scale_lo;                    // scale - (float)scale: the compensated periodic wrap
 };
 
 // Per-thread cell registers: 4 consecutive cells.
@@ -132,9 +140,10 @@ struct PlaceCellRegs {
   float cx[4], cy[4], k[4];
   float fc[WI > 0 ? WI : 1][4], tc[WI > 0 ? WI : 1][4], tq[WI > 0 ? WI : 1][4];   // tq = 1 - tc
   float ce0[4], ce1[4];
+  float cxl[4], cyl[4];              // COMP only: residuals of the centred centres
 };
 
-template <int WI>
+template <int WI, bool COMP = false>
 RIAB_DEV void place_load_cells(PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0) {
   const float* base = c.packed;
   const int np = c.n_pad;
@@ -162,6 +171,10 @@ RIAB_DEV void place_load_cells(PlaceCellRegs<WI>& r, const PlaceConst& c, int ce
   if (WI > 0 && c.geometry == RIAB_GEOM_GEODESIC) {
     ldv(r.ce0, base + (4 + 2 * c.n_inner) * np + cell0);
     ldv(r.ce1, base + (5 + 2 * c.n_inner) * np + cell0);
+  }
+  if (COMP) {
+    ldv(r.cxl, base + (6 + 2 * c.n_inner) * np + cell0);
+    ldv(r.cyl, base + (7 + 2 * c.n_inner) * np + cell0);
   }
 }
 
@@ -206,13 +219,25 @@ __device__ __noinline__ unsigned place_blocked_exact4(const double* __restrict__
   return m;
 }
 
+// |p' - c'| along one axis in the periodic box, compensated: s + e = (p - c) exactly up to the residuals' rounding, with
+// e the two-difference residual of s = p_hi - c_hi plus lo = p_lo - c_lo; the wrapped (scale - |p - c|) is formed as
+// (scale_f - |s|) + (scale_lo - sign(s) e), whose first term is exact near the wrap (Sterbenz).
+RIAB_DEV float periodic_comp(float p, float cc, float lo, const PlaceConst& c) {
+  const float s = p - cc, b = s - p;
+  const float e = ((p - (s - b)) - (cc + b)) + lo;
+  const float d = fabsf(s + e);
+  return (d > c.half_f) ? (c.scale_f - fabsf(s)) + (c.scale_lo - (s < 0.f ? -e : e)) : d;
+}
+
 // Rates of one agent for this thread's 4 cells (branch-free fast path).
 //   rec     : the agent's record in shared memory (broadcast reads); holds the float64 position too
 //   inner_s : shared-memory offset of the float64 inner walls (exact fall-back only)
 //   unsure  : DEFER = true only ORs the band test into it -- the caller redoes the agents it covers
 //             later with DEFER = false, which tests per agent and takes the exact float64 path at once.
 //   EXP     : 1 = the expanded Gaussian form is known to be on (no branch), 0 = known off, -1 = test c.expanded
-template <int WI, int DESC, bool DEFER, int EXP = -1>
+//   COMP    : direct form with the float32 residuals of p' (record ep0 / ep1) and c' (cxl / cyl):
+//             dx = (px - cx) + (pxl - cxl), so |p'| and |c'| no longer limit the accuracy of d (PlaceConst::comp)
+template <int WI, int DESC, bool DEFER, int EXP = -1, bool COMP = false>
 RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0,
                            const float* __restrict__ rec, uint32_t inner_s, bool& unsure_io) {
   const float4 r0 = *reinterpret_cast<const float4*>(rec);          // px, py, ep0 | -k|p|^2, ep1
@@ -269,7 +294,7 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
   // ---- Gaussian with one common width, expanded:  -k|c-p|^2 = (-k|c|^2 - k|p|^2) + (2k cx) px + (2k cy) py.
   // 1 FADD + 2 FFMA per rate on per-cell registers (2k cx, 2k cy, -k|c|^2); only used when k * r2_max <= 10,
   // where the cancellation costs < 4e-6 relative (make_place).  Blocked pairs: exponent - 1e5 -> rate 0 (d = 1000).
-  if (DESC == RIAB_PC_GAUSSIAN && (EXP >= 1 || (EXP < 0 && c.expanded))) {
+  if (!COMP && DESC == RIAB_PC_GAUSSIAN && (EXP >= 1 || (EXP < 0 && c.expanded))) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {                         // cell pairs: FADD + 2 (3) FFMA per rate
       float t0 = fmaf(r.cy[2 * h], r0.y, fmaf(r.cx[2 * h], r0.x, r.k[2 * h] + r0.z));
@@ -285,15 +310,24 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
   if (WI == 0 && c.periodic) {                           // warp-uniform
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      float dx = fabsf(r0.x - r.cx[i]), dy = fabsf(r0.y - r.cy[i]);
-      dx = (dx > c.half_f) ? c.scale_f - dx : dx;        // the short way round
-      dy = (dy > c.half_f) ? c.scale_f - dy : dy;
+      float dx, dy;
+      if (COMP) {
+        // the wrapped distance scale - |dx| is small where |dx| is large: the rounding of px - cx itself counts there, so
+        // it is kept as the exact residual of the difference (two-difference), and scale's own float32 residual added
+        dx = periodic_comp(r0.x, r.cx[i], r0.z - r.cxl[i], c);
+        dy = periodic_comp(r0.y, r.cy[i], r0.w - r.cyl[i], c);
+      } else {
+        dx = fabsf(r0.x - r.cx[i]); dy = fabsf(r0.y - r.cy[i]);
+        dx = (dx > c.half_f) ? c.scale_f - dx : dx;      // the short way round
+        dy = (dy > c.half_f) ? c.scale_f - dy : dy;
+      }
       d2[i] = fmaf(dy, dy, dx * dx);
     }
   } else {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const float dx = r0.x - r.cx[i], dy = r0.y - r.cy[i];
+      const float dx = COMP ? (r0.x - r.cx[i]) + (r0.z - r.cxl[i]) : r0.x - r.cx[i];
+      const float dy = COMP ? (r0.y - r.cy[i]) + (r0.w - r.cyl[i]) : r0.y - r.cy[i];
       d2[i] = fmaf(dy, dy, dx * dx);
     }
   }
@@ -325,7 +359,7 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
     if (desc == RIAB_PC_TOP_HAT) {
       // Neurons.py:975-976: 1*(dist < widths) with the scalar `widths`
       bool in = dv < c.top_hat_w2;
-      if (fabsf(dv - c.top_hat_w2) < 4e-6f * (c.top_hat_w2 + 1e-3f) && !blocked) {
+      if (fabsf(dv - c.top_hat_w2) < c.top_hat_band && !blocked) {
         const int cell = cell0 + i;
         if (cell < c.n_cells) {
           const double2 p64 = *reinterpret_cast<const double2*>(rec + place_pos64(WI));

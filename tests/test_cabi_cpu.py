@@ -64,10 +64,46 @@ def test_place_pack_matches_numpy():
     assert np.allclose(np.abs(fc), np.abs(centres[:, 0] - 0.3), atol=1e-6)
     assert np.allclose(tc, centres[:, 1] / 0.5, atol=1e-6)
     assert meta.eps[0] > 0 and meta.eps[1] > 0
+    # float32 residuals of the centred centres (compensated direct form), after ce0 / ce1: cx + cxl is the float64 value
+    cxl, cyl = out[10 * npad:10 * npad + n], out[11 * npad:11 * npad + n]
+    for j, res in ((0, cxl), (1, cyl)):
+        c = centres[:, j] - 0.5
+        assert np.array_equal(res, (c - c.astype(np.float32)).astype(np.float32))
+        assert np.abs(out[j * npad:j * npad + n].astype(float) + res - c).max() <= 2.0 ** -48
+    assert nfl == npad * (4 + 2 * 2 + 4)
     # bad arguments are refused with a message, not a crash
     assert lib.riab_place_pack(None, f(widths), n, f(walls), 6, 4, f(ext), 1, C.byref(meta),
                                out.ctypes.data_as(_lib.c_float_p)) < 0
     assert b"riab_place_pack" in lib.riab_last_error()
+
+
+def test_grid_pack_switches_to_turns_for_large_boxes():
+    """riab_grid_pack keeps radians while |k| r_max <= 40 (the default grid scales in the unit box) and packs wave vectors
+    and phases in turns beyond (scale 10), for the kernel's compensated phase; both give the oracle's phases."""
+    from ratinabox_b200 import _lib
+    lib = _lib.load()
+    rs = np.random.RandomState(2)
+    n = 12
+    gs, th, ph = rs.choice([0.3, 0.5, 0.8], n), rs.uniform(0, 1, n), rs.uniform(-300, 300, (n, 2))
+    w = O.grid_cells_w(th)
+    f = lambda a: np.ascontiguousarray(a).ctypes.data_as(_lib.c_double_p)
+    for scale, turns in ((1.0, 0), (2.5, 0), (10.0, 1)):
+        ext = np.array([0.0, scale, 0.0, scale])
+        meta = _lib.GridCells()
+        out = np.zeros(lib.riab_grid_pack_floats(n), dtype=np.float32)
+        assert lib.riab_grid_pack(f(gs), f(ph), f(w), n, f(ext), C.byref(meta), out.ctypes.data_as(_lib.c_float_p)) == 0
+        assert meta.phase_turns == turns
+        npad, unit = meta.n_pad, (2 * np.pi if turns else 1.0)
+        origin = gs[:, None] * ph / (2 * np.pi)
+        for p in np.array([[0.93, 0.07], [0.0, 1.0], [1.0, 0.0], [0.5, 0.5]]) * scale:
+            q = p - scale / 2
+            for k in range(3):
+                kx, ky, ph0 = (out[(3 * k + j) * npad:(3 * k + j) * npad + n].astype(float) * unit for j in range(3))
+                phi = ph0 - (q[0] * kx + q[1] * ky)
+                ref = (2 * np.pi / gs) * ((origin - p) * w[:, k, :]).sum(axis=1)
+                # each packed value rounded once from float64: at most 2^-24 of |kx q_x|, |ky q_y| and |ph0| each
+                bound = 2.0 ** -24 * (np.abs(kx * q[0]) + np.abs(ky * q[1]) + np.abs(ph0)) * (1 + 1e-6) + 1e-12
+                assert (np.abs(np.remainder(phi - ref + np.pi, 2 * np.pi) - np.pi) <= bound).all(), (scale, k)
 
 
 def test_grid_and_bvc_pack():
