@@ -215,6 +215,58 @@ typedef struct {
 /* fwd_prm: the forward agent's motion parameters, dt = lead dt * v_sequence / average_measured_speed. */
 int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const riab_motion_params* fwd_prm, void* stream);
 
+/* ------------------------------------------------- DumbAgent, ShiftAgent, ReplayAgent
+ * contribs/SubAgent.py:118-179, :358-431, :466-478: the position of one SubAgent per lead agent at one lead step,
+ * written to out_pos; the SubAgent then moves there with riab_agent_update_src (RIAB_MOTION_FORCED).  float64, in the
+ * reference's operation order.
+ *   RIAB_SUBAGENT_SHIFT  lead pos + lead head direction * shift_m (no boundary condition, :476)
+ *   RIAB_SUBAGENT_DUMB   :151-179: OU + spring on displacement_velocity, displacement cut back to 0.95 of the nearest
+ *                        strict wall crossing of [lead pos, lead pos + displacement], boundary conditions (a polygon or
+ *                        hole re-draws a random position), displacement re-measured through the boundary
+ *   RIAB_SUBAGENT_REPLAY :380-426: not replaying: one uniform, u > p_start tracks the lead, else a replay starts at a
+ *                        random position of the sham agent; replaying with t < end: the sham's rollout interpolated by
+ *                        its distance at replay_speed (t - start), the rollout stepped lazily with motion_step
+ *                        (sham_prm) while its distance is below the query and the stop; else back to the lead.
+ * Draws: Philox4x32-10 keyed by global agent id; DUMB: stream 6 (sub 0 the two normals, sub 1 + k the k-th re-draw),
+ * step = `step`; REPLAY: stream 7 (sub 0: u, speed; sub 1: duration, direction; sub 2 + k: the k-th start position),
+ * step = `step`; rollouts: stream 8, sub = the agent's replay index, step = rollout step. */
+typedef enum { RIAB_SUBAGENT_SHIFT = 0, RIAB_SUBAGENT_DUMB = 1, RIAB_SUBAGENT_REPLAY = 2 } riab_subagent_kind;
+#define RIAB_REPLAY_FIELDS 9          /* replay_state columns: speed, duration, start, end, stop, start distance,
+                                         previous rollout sample's distance, x, y */
+typedef struct {
+  int64_t n_agents;
+  int64_t id_offset;                  /* global id of row 0 */
+  int32_t kind;                       /* riab_subagent_kind */
+  int32_t reserved;
+  uint64_t seed;
+  uint64_t step;                      /* this SubAgent's update count (Philox step word) */
+  const double* lead_pos;             /* (A,2) device: the lead Agent's state after its update */
+  const double* lead_head_direction;  /* (A,2) SHIFT */
+  double dt;                          /* LeadAgent.dt */
+  double shift_m;                     /* SHIFT */
+  /* DUMB */
+  double* displacement;               /* (A,2) in / out */
+  double* displacement_velocity;      /* (A,2) in / out */
+  double ou_theta, ou_sigma;          /* 1 / tau_v, sqrt(2 sigma^2 / (tau_v dt)) (utils.py:364-366) */
+  double acceleration_scale;
+  const double* xi_displacement;      /* (A,2) injected standard normals or NULL */
+  const double* resample_pos;         /* (A,2) injected re-drawn positions or NULL */
+  /* REPLAY */
+  double t;                           /* the ReplayAgent's t before the step (:399) */
+  double p_start;                     /* replay_freq * dt */
+  double mean_speed, mean_duration;
+  uint8_t* replaying;                 /* (A) in / out: is_undergoing_replay */
+  double* replay_state;               /* (A, RIAB_REPLAY_FIELDS) */
+  int64_t* replay_count;              /* (A,2): replays started, rollout steps of the current one */
+  riab_agents sham;                   /* the sham rollout agent's state (n_agents, id_offset ignored) */
+  const double* replay_draws;         /* (A,6) injected u, speed, duration (before the clamp), x0, y0, direction or NULL */
+  const double* xi_replay;            /* (A, xi_steps, 2) injected standard normals of rollout steps 0.. or NULL */
+  int64_t xi_steps;
+  double* out_pos;                    /* (A,2) device */
+} riab_subagent;
+/* sham_prm: the sham agent's motion parameters (REPLAY; may be NULL otherwise). */
+int riab_subagent_step(const riab_subagent* sa, const riab_env* env, const riab_motion_params* sham_prm, void* stream);
+
 /* ----------------------------------------------------------------- PlaceCells */
 typedef enum { RIAB_PC_GAUSSIAN = 0, RIAB_PC_GAUSSIAN_THRESHOLD = 1, RIAB_PC_DIFF_OF_GAUSSIANS = 2,
                RIAB_PC_TOP_HAT = 3, RIAB_PC_ONE_HOT = 4 } riab_pc_description;   /* Neurons.py:959-976 */

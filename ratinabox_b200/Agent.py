@@ -71,6 +71,7 @@ class _HistoryView:
 
 
 class Agent:
+    _VEC_NAMES = _VEC          # state arrays with a trailing axis of 2 (a subclass may keep more arrays in self._s)
     default_params = {                                              # ratinabox/Agent.py:68-84
         "name": None,
         "dt": 0.05,
@@ -212,7 +213,7 @@ class Agent:
     def _squeeze(self, name, arr):
         if self.n_agents != 1:
             return arr
-        return arr[0].copy() if name in _VEC else arr[0].item()
+        return arr[0].copy() if name in self._VEC_NAMES else arr[0].item()
 
     _SHADOW_MAX = 4096      # above this many agents state reads are plain copies (no in-place write tracking)
 
@@ -277,7 +278,7 @@ class Agent:
         if name == "pos":
             self._wait_pos_copy()
         arr = np.asarray(value, dtype=np.float64)
-        if name in _VEC:
+        if name in self._VEC_NAMES:
             arr = np.broadcast_to(arr.reshape(-1, 2) if arr.size == 2 * self.n_agents else arr, (self.n_agents, 2))
         else:
             arr = np.broadcast_to(arr.reshape(-1) if arr.size == self.n_agents else arr, (self.n_agents,))

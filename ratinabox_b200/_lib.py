@@ -69,6 +69,21 @@ class ThetaSeq(C.Structure):
 THETA_NONE, THETA_BEHIND, THETA_AHEAD_FIRST, THETA_AHEAD = 0, 1, 2, 3   # riab_theta_phase
 
 
+class SubAgentStep(C.Structure):
+    _fields_ = [("n_agents", C.c_int64), ("id_offset", C.c_int64), ("kind", C.c_int32), ("reserved", C.c_int32),
+                ("seed", C.c_uint64), ("step", C.c_uint64), ("lead_pos", C.c_void_p), ("lead_head_direction", C.c_void_p),
+                ("dt", C.c_double), ("shift_m", C.c_double), ("displacement", C.c_void_p),
+                ("displacement_velocity", C.c_void_p), ("ou_theta", C.c_double), ("ou_sigma", C.c_double),
+                ("acceleration_scale", C.c_double), ("xi_displacement", C.c_void_p), ("resample_pos", C.c_void_p),
+                ("t", C.c_double), ("p_start", C.c_double), ("mean_speed", C.c_double), ("mean_duration", C.c_double),
+                ("replaying", C.c_void_p), ("replay_state", C.c_void_p), ("replay_count", C.c_void_p), ("sham", Agents),
+                ("replay_draws", C.c_void_p), ("xi_replay", C.c_void_p), ("xi_steps", C.c_int64), ("out_pos", C.c_void_p)]
+
+
+SUBAGENT_SHIFT, SUBAGENT_DUMB, SUBAGENT_REPLAY = 0, 1, 2       # riab_subagent_kind
+REPLAY_FIELDS = 9                                            # RIAB_REPLAY_FIELDS
+
+
 class PlaceCells(C.Structure):
     _fields_ = [("n_cells", C.c_int32), ("description", C.c_int32), ("wall_geometry", C.c_int32),
                 ("n_inner_walls", C.c_int32), ("min_fr", C.c_float), ("max_fr", C.c_float),
@@ -199,6 +214,7 @@ SYMBOLS = {
     "riab_agent_update_src": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                         C.POINTER(MotionSource), C.c_void_p]),
     "riab_theta_seq_step": (C.c_int, [C.POINTER(ThetaSeq), C.POINTER(Env), C.POINTER(MotionParams), C.c_void_p]),
+    "riab_subagent_step": (C.c_int, [C.POINTER(SubAgentStep), C.POINTER(Env), C.POINTER(MotionParams), C.c_void_p]),
     "riab_place_pack_floats": (C.c_int64, [C.c_int32, C.c_int32]),
     "riab_place_pack": (C.c_int, [c_double_p, c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_int32, c_double_p,
                                   C.c_int32, C.POINTER(PlaceCells), c_float_p]),

@@ -1,4 +1,5 @@
-"""ratinabox.contribs.SubAgent (contribs/SubAgent.py:10-36) and ThetaSequenceAgent (:182-356) on the device.
+"""ratinabox.contribs.SubAgent (contribs/SubAgent.py:10-36), ThetaSequenceAgent (:182-356), DumbAgent (:118-179),
+ReplayAgent (:358-431), ShiftAgent (:466-478) and UnrelatedAgent (:480-489) on the device.
 
 A SubAgent is an Agent over the same batch as its lead Agent (same ``n_agents``, ``id_offset`` and ``dt``) whose
 ``update()`` follows the lead's.  ThetaSequenceAgent's position is a theta sweep over the lead's: once per theta cycle it
@@ -14,7 +15,13 @@ Where the reference raises, this returns a defined position instead (DESIGN.md, 
 The forward rollout is stepped lazily, only as far as the sweep has reached, which gives the reference's interpolated
 positions bit for bit with no bound on the number of rollout steps.  ``run()`` is not available: the lead's whole-run
 kernel does not drive SubAgents.
+
+DumbAgent, ShiftAgent and ReplayAgent make one riab_subagent_step launch per ``update()`` (the position of every agent,
+float64 in the reference's operation order) followed by the same forced step; UnrelatedAgent is an Agent stepped with
+the lead's dt.  ReplayAgent rolls its sham agent out lazily, like the ThetaSequenceAgent's look ahead (DESIGN.md,
+SubAgents).
 """
+import math
 import copy
 import ctypes as C
 import warnings
@@ -219,3 +226,267 @@ class ThetaSequenceAgent(SubAgent):
         self.last_theta_phase = theta_phase       # :345-346
         self.counter += 1
         SubAgent.update(self, forced_next_position=self._out)
+
+
+def _tensor_tap(agent, value, shape):
+    """A parity tap (injected draws) as a contiguous float64 device tensor of `shape`, or None."""
+    import torch
+    if value is None:
+        return None
+    return torch.as_tensor(np.ascontiguousarray(value, dtype=np.float64), device=agent.device).reshape(shape)
+
+
+class DumbAgent(SubAgent):
+    """ratinabox.contribs.SubAgent.DumbAgent (contribs/SubAgent.py:118-179): the lead's position plus a displacement on a
+    stochastic spring.  Per step the displacement velocity takes an Ornstein-Uhlenbeck step (noise sigma, timescale tau_v)
+    plus the spring's -acceleration_scale * displacement * dt; a displacement that crosses a wall is cut back to 0.95 of
+    the nearest crossing; the boundary conditions apply, and the displacement is re-measured through the environment.
+
+    ``displacement`` and ``displacement_velocity`` are (n_agents, 2) float64 device state, read and written like the
+    Agent's own state arrays.  ``sigma``, ``tau_v`` and ``acceleration_scale`` are fixed at construction, as in the
+    reference.
+    """
+    default_params = {                                              # contribs/SubAgent.py:134-136
+        "drift_distance": 0.05,
+        "drift_timescale": 3.0,
+    }
+    _VEC_NAMES = Agent._VEC_NAMES | {"displacement", "displacement_velocity"}
+
+    def __init__(self, LeadAgent, params={}):
+        import torch
+        p = copy.deepcopy(__class__.default_params)
+        p.update(params)
+        super().__init__(LeadAgent, p)
+        f64 = dict(dtype=torch.float64, device=self.device)
+        self._s["displacement"] = torch.zeros((self.n_agents, 2), **f64)            # :145-146
+        self._s["displacement_velocity"] = torch.zeros((self.n_agents, 2), **f64)
+        self.tau_v = self.drift_timescale / 2                                         # :147-149
+        self.sigma = np.pi**2 * self.drift_distance / (self.drift_timescale**2)
+        self.acceleration_scale = self.sigma / self.drift_distance
+        self._sa = _lib.SubAgentStep()
+        self._out = torch.empty((self.n_agents, 2), **f64)
+        self._updates = 0
+
+    displacement = property(lambda self: self._get_state("displacement"),
+                            lambda self, v: self._set_state("displacement", v))
+    displacement_velocity = property(lambda self: self._get_state("displacement_velocity"),
+                                     lambda self, v: self._set_state("displacement_velocity", v))
+
+    def update(self, **kwargs):
+        """DumbAgent.update (contribs/SubAgent.py:151-179) for every agent.  Parity taps: ``_xi_displacement``
+        (n_agents, 2) standard normals of the OU step, ``_resample_pos`` (n_agents, 2) the positions a polygon or hole
+        re-draws."""
+        Lead = self.LeadAgent
+        lead = _current_state(Lead)
+        self._flush_pending()
+        self._sync_user_writes()
+        dt = float(Lead.dt)
+        xi = _tensor_tap(self, kwargs.get("_xi_displacement"), (self.n_agents, 2))
+        rs = _tensor_tap(self, kwargs.get("_resample_pos"), (self.n_agents, 2))
+        sa = self._sa
+        sa.n_agents, sa.id_offset, sa.kind = self.n_agents, int(self.id_offset), _lib.SUBAGENT_DUMB
+        sa.seed, sa.step = int(self.seed) & 0xFFFFFFFFFFFFFFFF, self._updates
+        sa.lead_pos, sa.dt = lead["pos"].data_ptr(), dt
+        sa.displacement, sa.displacement_velocity = self._s["displacement"].data_ptr(), self._s["displacement_velocity"].data_ptr()
+        s = float(self.sigma)                                          # utils.ornstein_uhlenbeck (utils.py:363-366)
+        sa.ou_theta = 1 / float(self.tau_v)
+        sa.ou_sigma = math.sqrt((2 * (s * s)) / (float(self.tau_v) * dt))
+        sa.acceleration_scale = float(self.acceleration_scale)
+        sa.xi_displacement = xi.data_ptr() if xi is not None else None
+        sa.resample_pos = rs.data_ptr() if rs is not None else None
+        sa.out_pos = self._out.data_ptr()
+        _lib.check(self._lib.riab_subagent_step(C.byref(sa), C.byref(self._env_struct()), None, self._stream()))
+        self._taps = (xi, rs)                     # the launch reads them asynchronously
+        self._updates += 1
+        SubAgent.update(self, forced_next_position=self._out)
+
+
+class ShiftAgent(SubAgent):
+    """ratinabox.contribs.SubAgent.ShiftAgent (contribs/SubAgent.py:466-478): the lead's position shifted by ``shift_m``
+    along the lead's head direction (negative: behind it).  No boundary condition applies, as in the reference: in a
+    periodic box the position may lie outside the box."""
+    default_params = {                                              # contribs/SubAgent.py:471-473
+        "shift_m": 0.01,
+    }
+
+    def __init__(self, LeadAgent, params={}):
+        import torch
+        p = copy.deepcopy(__class__.default_params)
+        p.update(params)
+        super().__init__(LeadAgent, p)
+        self._sa = _lib.SubAgentStep()
+        self._out = torch.empty((self.n_agents, 2), dtype=torch.float64, device=self.device)
+
+    def update(self, **kwargs):
+        """ShiftAgent.update (contribs/SubAgent.py:475-478) for every agent."""
+        lead = _current_state(self.LeadAgent)
+        self._flush_pending()
+        sa = self._sa
+        sa.n_agents, sa.id_offset, sa.kind = self.n_agents, int(self.id_offset), _lib.SUBAGENT_SHIFT
+        sa.lead_pos, sa.lead_head_direction = lead["pos"].data_ptr(), lead["head_direction"].data_ptr()
+        sa.shift_m = float(self.shift_m)
+        sa.out_pos = self._out.data_ptr()
+        _lib.check(self._lib.riab_subagent_step(C.byref(sa), C.byref(self._env_struct()), None, self._stream()))
+        SubAgent.update(self, forced_next_position=self._out)
+
+
+def _replay_attr(name, col):
+    """A ReplayAgent attribute the reference overwrites per replay: the (n_agents,) device column (a scalar when
+    n_agents == 1).  Before the device state exists (construction) it holds the parameter's value."""
+    def get(self):
+        if "_replay_state" not in self.__dict__:
+            return self.__dict__["_init_" + name]
+        v = self._replay_state[:, col].cpu().numpy()
+        return float(v[0]) if self.n_agents == 1 else v
+
+    def set(self, v):
+        if "_replay_state" in self.__dict__:
+            raise AttributeError(f"ReplayAgent.{name} is per-agent device state and is read-only")
+        self.__dict__["_init_" + name] = v
+    return property(get, set)
+
+
+class ReplayAgent(SubAgent):
+    """ratinabox.contribs.SubAgent.ReplayAgent (contribs/SubAgent.py:358-431): tracks the lead, except during replays.
+    While not replaying, each agent starts a replay with probability replay_freq * dt per step: it jumps to a random
+    position and follows a fresh random-motion trajectory of a sham agent at a Rayleigh-drawn ``replay_speed`` (mean
+    parameter ``replay_speed``) for a Rayleigh-drawn ``replay_duration`` (at least half its mean parameter), then returns
+    to the lead.
+
+    The sham agent's rollout is stepped lazily on the device, only as far as each step's query, which gives the
+    reference's interpolated positions with O(1) state per agent.  The sham agent moves with this agent's motion
+    parameters and the lead's dt; it is not registered in the Environment.  ``is_undergoing_replay``,
+    ``replay_speed``, ``replay_duration``, ``replay_start_time`` and ``replay_end_time`` are read-only (n_agents,)
+    arrays (scalars when n_agents == 1); ``history["replay"]`` holds the replay flag after each step.
+    """
+    default_params = {                                              # contribs/SubAgent.py:360-364
+        "replay_freq": 0.3,
+        "replay_duration": 0.1,
+        "replay_speed": 1.0,
+    }
+    replay_speed = _replay_attr("replay_speed", 0)
+    replay_duration = _replay_attr("replay_duration", 1)
+    replay_start_time = _replay_attr("replay_start_time", 2)
+    replay_end_time = _replay_attr("replay_end_time", 3)
+
+    def __init__(self, LeadAgent, params={}):
+        import torch
+        p = copy.deepcopy(__class__.default_params)
+        p.update(params)
+        super().__init__(LeadAgent, p)
+        A = self.n_agents
+        self.mean_replay_speed = self.replay_speed                                   # :370-373
+        self.mean_replay_duration = self.replay_duration
+        f64 = dict(dtype=torch.float64, device=self.device)
+        state = torch.full((A, _lib.REPLAY_FIELDS), float("nan"), **f64)
+        state[:, 0], state[:, 1] = float(self.mean_replay_speed), float(self.mean_replay_duration)
+        self._replaying = torch.zeros(A, dtype=torch.uint8, device=self.device)
+        self._replay_count = torch.zeros((A, 2), dtype=torch.int64, device=self.device)
+        self._flags = None                        # (history capacity, A) uint8, rows aligned with the history ring's
+        # the sham agent (:376-378): Agent.__init__'s initial state; its measured velocity, head direction and distance
+        # carry over between replays
+        pos = self.Environment.sample_positions(n=A, method="random")
+        direction = np.random.uniform(0, 2 * np.pi, size=A)
+        vel = self.speed_mean * np.stack((np.cos(direction), np.sin(direction)), axis=1)
+        self._sham = {k: torch.zeros_like(self._s[k]) for k in _STATE}
+        self._sham["pos"].copy_(torch.as_tensor(pos, **f64))
+        self._sham["velocity"].copy_(torch.as_tensor(vel, **f64))
+        self._sham["measured_velocity"].copy_(torch.as_tensor(vel, **f64))
+        self._sham["head_direction"].copy_(torch.as_tensor(vel / np.linalg.norm(vel, axis=1, keepdims=True), **f64))
+        self._sham["distance_to_closest_wall"].fill_(float("inf"))
+        self._sham_c = _lib.Agents()
+        self._sham_c.n_agents, self._sham_c.id_offset = A, int(self.id_offset)
+        for k in _STATE:
+            setattr(self._sham_c, k, self._sham[k].data_ptr())
+        self._sham_mp = _lib.MotionParams()
+        self._sa = _lib.SubAgentStep()
+        self._out = torch.empty((A, 2), **f64)
+        self._updates = 0
+        self._replay_state = state                # from here on the replay attributes read the device
+
+    @property
+    def is_undergoing_replay(self):
+        v = self._replaying.cpu().numpy().astype(bool)
+        return bool(v[0]) if self.n_agents == 1 else v
+
+    def update(self, **kwargs):
+        """ReplayAgent.update (contribs/SubAgent.py:380-426) for every agent.  Parity taps: ``_replay_draws``
+        (n_agents, 6) = the uniform, replay_speed, the Rayleigh duration before its clamp, the start position (x, y) and
+        the start direction, used by agents that are not replaying; ``_xi_replay`` (n_agents, K, 2) standard normals of
+        rollout steps 0..K-1 of the current replay."""
+        t_before = float(self.t)                   # :399 reads self.t before SubAgent.update sets it
+        lead = _current_state(self.LeadAgent)
+        self._flush_pending()
+        self._sync_user_writes()
+        A = self.n_agents
+        draws = _tensor_tap(self, kwargs.get("_replay_draws"), (A, 6))
+        xi = kwargs.get("_xi_replay")
+        xi = _tensor_tap(self, xi, (A, -1, 2)) if xi is not None else None
+        self._fill_motion_params(self.dt, {}, mp=self._sham_mp)
+        sa = self._sa
+        sa.n_agents, sa.id_offset, sa.kind = A, int(self.id_offset), _lib.SUBAGENT_REPLAY
+        sa.seed, sa.step = int(self.seed) & 0xFFFFFFFFFFFFFFFF, self._updates
+        sa.lead_pos, sa.dt, sa.t = lead["pos"].data_ptr(), float(self.dt), t_before
+        sa.p_start = self.replay_freq * self.dt
+        sa.mean_speed, sa.mean_duration = float(self.mean_replay_speed), float(self.mean_replay_duration)
+        sa.replaying, sa.replay_state = self._replaying.data_ptr(), self._replay_state.data_ptr()
+        sa.replay_count, sa.sham = self._replay_count.data_ptr(), self._sham_c
+        sa.replay_draws = draws.data_ptr() if draws is not None else None
+        sa.xi_replay, sa.xi_steps = (xi.data_ptr(), int(xi.shape[1])) if xi is not None else (None, 0)
+        sa.out_pos = self._out.data_ptr()
+        _lib.check(self._lib.riab_subagent_step(C.byref(sa), C.byref(self._env_struct()), C.byref(self._sham_mp),
+                                                self._stream()))
+        self._taps = (draws, xi)                  # the launch reads them asynchronously
+        self._updates += 1
+        SubAgent.update(self, forced_next_position=self._out)
+        if self.save_history:                     # save_to_history (:428-431): the flag after this step
+            self._flag_row().copy_(self._replaying)
+
+    def _flag_row(self):
+        """The flag ring's row of the history row this step wrote; the ring grows with the Agent's (same capacity,
+        rows copied the same way), so its rows wrap in lockstep."""
+        import torch
+        cap = self._hist_cap
+        if self._flags is None or self._flags.shape[0] != cap:
+            new = torch.zeros((cap, self.n_agents), dtype=torch.uint8, device=self.device)
+            if self._flags is not None:
+                new[: self._flags.shape[0]].copy_(self._flags)
+            self._flags = new
+        return self._flags[(self._hist_rows - 1) % cap]
+
+    def _history_keys(self):
+        return super()._history_keys() + ["replay"]
+
+    def get_history_arrays(self):
+        """Agent.get_history_arrays plus ``replay``: bool (T,), or (T, n_agents) with more than one agent."""
+        import torch
+        fresh = self._last_history_array_cache_time != (self.t, self._hist_rows)
+        arrays = super().get_history_arrays()
+        if fresh or "replay" not in arrays:
+            n = min(self._hist_rows, self._hist_cap)
+            if n == 0 or self._flags is None:
+                flags = np.zeros((n, self.n_agents), dtype=bool)
+            else:
+                start = self._hist_rows % self._hist_cap if self._hist_rows > self._hist_cap else 0
+                idx = (torch.arange(n, device=self.device) + start) % self._hist_cap
+                flags = self._flags[idx].cpu().numpy().astype(bool)
+            arrays["replay"] = flags[:, 0] if self.n_agents == 1 else flags
+        return arrays
+
+
+class UnrelatedAgent(SubAgent):
+    """ratinabox.contribs.SubAgent.UnrelatedAgent (contribs/SubAgent.py:480-489): an independent random walker with the
+    lead's dt (and its batch).  It starts from the lead's position and velocity, so with the lead's seed it would repeat
+    the lead's path step for step; without a ``seed`` parameter it takes one derived from the lead's."""
+    default_params = {}
+
+    def __init__(self, LeadAgent, params={}):
+        p = dict(params)
+        if "seed" not in p:
+            p["seed"] = (int(LeadAgent.seed) * 0x9E3779B97F4A7C15 + 0x554E52454C) & 0xFFFFFFFFFFFFFFFF
+        super().__init__(LeadAgent, p)
+
+    def update(self, **kwargs):
+        """SubAgent.update() (contribs/SubAgent.py:487-489): the random-motion step; Agent.update's parity tap ``_xi``
+        passes through."""
+        SubAgent.update(self, **kwargs)

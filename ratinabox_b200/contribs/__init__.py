@@ -2,4 +2,5 @@ from .TaskEnvironment import SpatialGoalEnvironment  # noqa: F401
 from .ValueNeuron import ValueNeuron  # noqa: F401
 from .SuccessorFeatures import SuccessorFeatures  # noqa: F401
 from .PhasePrecessingPlaceCells import PhasePrecessingPlaceCells  # noqa: F401
-from .SubAgent import SubAgent, ThetaSequenceAgent  # noqa: F401
+from .SubAgent import (SubAgent, ThetaSequenceAgent, DumbAgent, ReplayAgent, ShiftAgent,  # noqa: F401
+                       UnrelatedAgent)

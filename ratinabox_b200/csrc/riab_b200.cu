@@ -13,6 +13,7 @@
 //   k_bvc_integrate     BVC phase B (float32 angular integral, TMA-staged tables)
 //   k_td_*              TD learning of ValueNeuron / SuccessorFeatures (riab_td.cuh)
 //   k_theta_seq         ThetaSequenceAgent sweep positions over a lead Agent's batch, one agent per thread (float64)
+//   k_subagent          DumbAgent / ShiftAgent / ReplayAgent positions over a lead Agent's batch, one agent per thread (float64)
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -36,6 +37,7 @@
 #include "riab_traj.cuh"
 #include "riab_td.cuh"
 #include "riab_theta.cuh"
+#include "riab_subagent.cuh"
 
 using namespace riab;
 
@@ -2758,6 +2760,152 @@ int hostio(HostIo*& h) {
 }
 }  // namespace
 
+// ------------------------------------------------- DumbAgent, ShiftAgent, ReplayAgent
+// One agent per thread: the position of this lead step (riab_subagent.cuh).  A replaying ReplayAgent advances its sham
+// agent's rollout with motion_step in place.
+template <int KIND>
+__global__ void __launch_bounds__(128) k_subagent(const riab_subagent sa, const riab_motion_params mp, const MotionDerived md,
+                                                  const EnvK env) {
+  __shared__ __align__(16) double s_walls[MAXW * 4];
+  __shared__ uint64_t s_bar;
+  if (KIND != RIAB_SUBAGENT_SHIFT) stage_walls(s_walls, &s_bar, env);
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= sa.n_agents) return;
+  const double2 lp = reinterpret_cast<const double2*>(sa.lead_pos)[i];
+  const unsigned long long gid = (unsigned long long)(sa.id_offset + i);
+  double px = lp.x, py = lp.y;
+  if (KIND == RIAB_SUBAGENT_SHIFT) {                                  // SubAgent.py:476
+    const double2 hd = reinterpret_cast<const double2*>(sa.lead_head_direction)[i];
+    px = (D(lp.x) + D(hd.x) * D(sa.shift_m)).v;
+    py = (D(lp.y) + D(hd.y) * D(sa.shift_m)).v;
+  } else if (KIND == RIAB_SUBAGENT_DUMB) {                            // SubAgent.py:151-179
+    double2 d = reinterpret_cast<const double2*>(sa.displacement)[i];
+    double2 v = reinterpret_cast<const double2*>(sa.displacement_velocity)[i];
+    double n1, n2;
+    if (sa.xi_displacement != nullptr) {
+      n1 = sa.xi_displacement[2 * i]; n2 = sa.xi_displacement[2 * i + 1];
+    } else {
+      uint32_t c[4];
+      philox_ctr(c, gid, 0u, sa.step, RIAB_STREAM_DUMB, 0u);
+      philox_normals(c, sa.seed, n1, n2);
+    }
+    const D dt(sa.dt), theta(sa.ou_theta), sigma(sa.ou_sigma), a(sa.acceleration_scale);
+    dumb_spring(d.x, v.x, dt, theta, sigma, a, D(n1));
+    dumb_spring(d.y, v.y, dt, theta, sigma, a, D(n2));
+    dumb_wall_cut(lp.x, lp.y, d.x, d.y, s_walls, env.W);
+    D qx = D(lp.x) + D(d.x), qy = D(lp.y) + D(d.y);
+    if (sa.resample_pos != nullptr && env.polygon && !env_contains(qx.v, qy.v, s_walls, env.nb, env.h0, env.nh)) {
+      qx = D(sa.resample_pos[2 * i]); qy = D(sa.resample_pos[2 * i + 1]);
+    } else {
+      apply_boundary(qx, qy, env.ext, s_walls, env.periodic != 0, env.polygon != 0, env.nb, env.h0, env.nh,
+                     [&](uint32_t t, double& u1, double& u2) {
+                       subagent_uniforms(sa.seed, gid, 1u + t, sa.step, RIAB_STREAM_DUMB, u1, u2);
+                     });
+    }
+    D wx, wy;                                                         // :178, through the boundary when periodic
+    step_displacement(qx, qy, D(lp.x), D(lp.y), env.periodic != 0, env.scale, wx, wy);
+    reinterpret_cast<double2*>(sa.displacement)[i] = make_double2(wx.v, wy.v);
+    reinterpret_cast<double2*>(sa.displacement_velocity)[i] = v;
+    px = qx.v; py = qy.v;
+  } else {                                                            // SubAgent.py:391-423
+    uint8_t rep = sa.replaying[i];
+    double* st = sa.replay_state + (size_t)RIAB_REPLAY_FIELDS * i;
+    const double* tap = sa.replay_draws != nullptr ? sa.replay_draws + 6 * i : nullptr;
+    if (!rep) {
+      double u, u_speed;
+      if (tap != nullptr) { u = tap[0]; u_speed = 0.0; }
+      else subagent_uniforms(sa.seed, gid, 0u, sa.step, RIAB_STREAM_REPLAY, u, u_speed);
+      if (!(u > sa.p_start)) {                                       // :395-407: a replay starts
+        double u_dur, u_dir;
+        if (tap == nullptr) subagent_uniforms(sa.seed, gid, 1u, sa.step, RIAB_STREAM_REPLAY, u_dur, u_dir);
+        const double speed = tap ? tap[1] : rayleigh_of(sa.mean_speed, u_speed);
+        const double raw = tap ? tap[2] : rayleigh_of(sa.mean_duration, u_dur);
+        const double half = (D(sa.mean_duration) / D(2.0)).v;
+        const double duration = half > raw ? half : raw;              // max(rayleigh, mean / 2)
+        const double dir = tap ? tap[5] : (D(2.0 * M_PI) * D(u_dir)).v;   // np.random.uniform(0, 2 pi)
+        double x0, y0;
+        if (tap != nullptr) {
+          x0 = tap[3]; y0 = tap[4];
+        } else {
+          // sample_positions(n=1, "random") (Environment.py:561-600): uniform in the extent, re-drawn until inside
+          for (uint32_t k = 0; k < 1024u; ++k) {
+            double ux, uy;
+            subagent_uniforms(sa.seed, gid, 2u + k, sa.step, RIAB_STREAM_REPLAY, ux, uy);
+            x0 = (D(env.ext[0]) + D(env.ext[1] - env.ext[0]) * D(ux)).v;
+            y0 = (D(env.ext[2]) + D(env.ext[3] - env.ext[2]) * D(uy)).v;
+            if (!env.polygon || env_contains(x0, y0, s_walls, env.nb, env.h0, env.nh)) break;
+          }
+        }
+        // initialise_position_and_velocity (Agent.py:523-535); the sham's measured velocity, head direction and
+        // distance carry over from its previous replay
+        AgentState s;
+        load_agent(sa.sham, i, s);
+        s.px = x0; s.py = y0;
+        s.vx = (D(mp.speed_mean) * D(cos(dir))).v;
+        s.vy = (D(mp.speed_mean) * D(sin(dir))).v;
+        s.rot = 0.0;
+        store_agent(sa.sham, i, s);
+        st[0] = speed; st[1] = duration;
+        st[2] = sa.t; st[3] = (D(sa.t) + D(duration)).v;
+        st[4] = (D(s.dist) + D(1.1) * D(speed) * D(duration)).v;     // :408's stop distance
+        st[5] = s.dist;
+        st[6] = s.dist; st[7] = x0; st[8] = y0;
+        sa.replay_count[2 * i] += 1;
+        sa.replay_count[2 * i + 1] = 0;
+        rep = 1;
+        px = x0; py = y0;
+      }
+    } else {
+      // :416-418 while t < end: the query distance; on the step the replay ends (:420-423) the rollout is finished to
+      // its stop distance instead, as the reference's eager one was: the sham's state carries over into the next replay
+      const bool live = sa.t < st[3];
+      const double q = live ? (D(st[0]) * (D(sa.t) - D(st[2]))).v : INFINITY;
+      AgentState s;
+      load_agent(sa.sham, i, s);
+      long long k = sa.replay_count[2 * i + 1];
+      const unsigned long long r = (unsigned long long)(sa.replay_count[2 * i] - 1);
+      const double start = st[5], stop = st[4];
+      double d_prev = st[6], x_prev = st[7], y_prev = st[8];
+      const double f1 = __longlong_as_double((long long)sa.seed);
+      while ((live && k == 0) || ((D(s.dist) - D(start)).v < q && s.dist < stop)) {
+        d_prev = s.dist; x_prev = s.px; y_prev = s.py;
+        double n1, n2;
+        if (sa.xi_replay != nullptr && k < sa.xi_steps) {
+          n1 = sa.xi_replay[2 * (i * sa.xi_steps + k)];
+          n2 = sa.xi_replay[2 * (i * sa.xi_steps + k) + 1];
+        } else {
+          uint32_t c[4];
+          philox_ctr(c, gid, (uint32_t)r, (uint64_t)k, RIAB_STREAM_REPLAY_FWD, 0u);
+          philox_normals(c, sa.seed, n1, n2);
+        }
+        // exactly-zero displacement / polygon re-draw fall-backs: keyed by replay, step and agent
+        const double f2 = __longlong_as_double((long long)(((unsigned long long)k | (r << 32)) ^ (gid << 20) ^
+                                                           0x5245504c41590000ull));
+        motion_step<false>(s, s_walls, env.W, mp, md, env.ext, env.periodic != 0, env.scale, env.polygon != 0, env.nb, env.h0,
+                           env.nh, n1, n2, false, 0.0, 0.0, f1, f2, nullptr, nullptr, nullptr);
+        ++k;
+      }
+      store_agent(sa.sham, i, s);
+      sa.replay_count[2 * i + 1] = k;
+      st[6] = d_prev; st[7] = x_prev; st[8] = y_prev;
+      if (live) {
+        // interp1d over the distances relative to the start (:411-418) between the kept pair
+        const double lo = (D(d_prev) - D(start)).v, hi = (D(s.dist) - D(start)).v;
+        if (hi >= q && q >= lo) {
+          px = interp_linear(q, lo, hi, x_prev, s.px);
+          py = interp_linear(q, lo, hi, y_prev, s.py);
+        } else {
+          px = py = theta_nan();
+        }
+      } else {
+        rep = 0;                                                      // back to the lead
+      }
+    }
+    sa.replaying[i] = rep;
+  }
+  reinterpret_cast<double2*>(sa.out_pos)[i] = make_double2(px, py);
+}
+
 // ===========================================================================
 extern "C" {
 
@@ -2965,6 +3113,41 @@ int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const ria
   MotionDerived md;
   derive_motion(*fwd_prm, md);
   k_theta_seq<<<(unsigned)((ts->n_agents + 127) / 128), 128, 0, (cudaStream_t)stream>>>(*ts, *fwd_prm, md, ek);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------- DumbAgent, ShiftAgent, ReplayAgent (k_subagent: before extern "C")
+int riab_subagent_step(const riab_subagent* sa, const riab_env* env, const riab_motion_params* sham_prm, void* stream) {
+  EnvK ek;
+  int rc;
+  if (sa == nullptr) return fail(RIAB_ERR_INVALID, "riab_subagent_step: sa is NULL");
+  if ((rc = make_env(env, ek))) return rc;
+  if (sa->kind < RIAB_SUBAGENT_SHIFT || sa->kind > RIAB_SUBAGENT_REPLAY) return fail(RIAB_ERR_INVALID, "bad SubAgent kind %d", sa->kind);
+  if (sa->n_agents < 0) return fail(RIAB_ERR_INVALID, "n_agents < 0");
+  if (sa->n_agents == 0) return 0;
+  if (!sa->lead_pos || !sa->out_pos) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL array");
+  const unsigned grid = (unsigned)((sa->n_agents + 127) / 128);
+  MotionDerived md{};
+  riab_motion_params mp{};
+  if (sa->kind == RIAB_SUBAGENT_SHIFT) {
+    if (!sa->lead_head_direction) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL lead_head_direction");
+    k_subagent<RIAB_SUBAGENT_SHIFT><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, mp, md, ek);
+  } else if (sa->kind == RIAB_SUBAGENT_DUMB) {
+    if (!sa->displacement || !sa->displacement_velocity) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL displacement");
+    k_subagent<RIAB_SUBAGENT_DUMB><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, mp, md, ek);
+  } else {
+    if (sham_prm == nullptr) return fail(RIAB_ERR_INVALID, "riab_subagent_step: a ReplayAgent needs sham_prm");
+    if ((rc = check_motion(sham_prm))) return rc;
+    if (!sa->replaying || !sa->replay_state || !sa->replay_count) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL replay state");
+    riab_agents sham = sa->sham;
+    sham.n_agents = sa->n_agents;
+    if ((rc = check_agents(&sham))) return rc;
+    if (sa->xi_replay != nullptr && sa->xi_steps < 0) return fail(RIAB_ERR_INVALID, "xi_steps < 0");
+    derive_motion(*sham_prm, md);
+    k_subagent<RIAB_SUBAGENT_REPLAY><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, *sham_prm, md, ek);
+  }
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;

@@ -75,7 +75,10 @@ RIAB_DEV void philox_round_keys(uint32_t (&rk)[2 * R], unsigned long long seed) 
 // Stream ids (third counter word, top byte)
 enum : uint32_t { RIAB_STREAM_AGENT_OU = 0, RIAB_STREAM_CELL_NOISE = 1, RIAB_STREAM_SPIKES = 2, RIAB_STREAM_MEASURE = 3,
                   RIAB_STREAM_THIN = 4,            // thinned spikes: calls n = 0, 1, ... of a (row, 128-cell block), n in bits 16.. of the sub-index
-                  RIAB_STREAM_THETA_FWD = 5 };     // ThetaSequenceAgent forward rollouts: sub-index = rollout, step = rollout step
+                  RIAB_STREAM_THETA_FWD = 5,       // ThetaSequenceAgent forward rollouts: sub-index = rollout, step = rollout step
+                  RIAB_STREAM_DUMB = 6,            // DumbAgent: sub 0 = the displacement normals, 1 + k = k-th re-drawn position
+                  RIAB_STREAM_REPLAY = 7,          // ReplayAgent decisions: sub 0, 1 = uniforms, 2 + k = k-th start position
+                  RIAB_STREAM_REPLAY_FWD = 8 };    // ReplayAgent rollouts: sub-index = replay index, step = rollout step
 
 // counter = (agent id lo32, sub-index, step lo32, (step hi & 0xffff) | stream<<24 | population<<16)
 RIAB_HD void philox_ctr(uint32_t (&c)[4], uint64_t agent, uint32_t sub, uint64_t step, uint32_t stream, uint32_t pop) {

@@ -110,6 +110,34 @@ RIAB_DEV bool env_contains(double x, double y, const double* __restrict__ walls,
   return (n_hole == 0) || !edges_contain(x, y, walls + 4 * hole0, n_hole);
 }
 
+// Environment.apply_boundary_conditions (Environment.py:855-894) for a position that may have left the environment.
+// Polygon or holes: "just resample random position" (:890-893) -- uniform in the extent until inside, draw(t, u1, u2)
+// giving the t-th pair of uniforms (the position is kept if 1024 draws miss).  Rectangle: pos % extent when periodic
+// (:877-879), else clamped 0.01 inside (:880-889).
+template <class Draw>
+RIAB_DEV void apply_boundary(D& px, D& py, const double* __restrict__ ext, const double* __restrict__ walls, bool periodic,
+                             bool polygon, int n_poly, int hole0, int n_hole, Draw draw) {
+  if (polygon) {
+    if (!env_contains(px.v, py.v, walls, n_poly, hole0, n_hole)) {
+      for (uint32_t t = 0; t < 1024u; ++t) {
+        double u1, u2;
+        draw(t, u1, u2);
+        const double qx = ext[0] + u1 * (ext[1] - ext[0]);
+        const double qy = ext[2] + u2 * (ext[3] - ext[2]);
+        if (env_contains(qx, qy, walls, n_poly, hole0, n_hole)) { px = D(qx); py = D(qy); break; }
+      }
+    }
+  } else if (!((px.v > ext[0]) && (px.v < ext[1]) && (py.v > ext[2]) && (py.v < ext[3]))) {
+    if (periodic) {
+      px = D(np_mod(px.v, ext[1]));
+      py = D(np_mod(py.v, ext[3]));
+    } else {
+      px = D(fmin(fmax(px.v, ext[0] + 0.01), ext[1] - 0.01));
+      py = D(fmin(fmax(py.v, ext[2] + 0.01), ext[3] - 0.01));
+    }
+  }
+}
+
 // A pos / prev_pos pair's displacement; through the boundary when periodic (Environment.py:670-675)
 RIAB_DEV void step_displacement(D px, D py, D ppx, D ppy, bool periodic, double scale, D& stx, D& sty) {
   stx = px - ppx; sty = py - ppy;
@@ -296,27 +324,15 @@ RIAB_DEV void motion_step(AgentState& s, const double* __restrict__ walls, int W
   if (REC && n_iters_out != nullptr) *n_iters_out = iters;
 
   // ---- A7: still inside? else clamp (Environment.py:781-818, :880-889)
-  if (polygon) {
-    if (!env_contains(px.v, py.v, walls, n_poly, hole0, n_hole)) {
-      // Environment.py:890-893: "just resample random position" -- uniform in the extent until inside
-      // (the reference draws from np.random; a Philox stream keyed like the zero-displacement fall-back here)
-      const long long k1 = __double_as_longlong(fallback_n1), k2 = __double_as_longlong(fallback_n2);
-      for (uint32_t t = 0; t < 1024u; ++t) {
-        uint32_t c[4] = {(uint32_t)k2, (uint32_t)(k2 >> 32), 0x52534d50u + t, RIAB_STREAM_MEASURE << 24};
-        philox4x32_10(c, (uint32_t)k1, (uint32_t)(k1 >> 32));
-        const double qx = ext[0] + u01_53(c[0], c[1]) * (ext[1] - ext[0]);
-        const double qy = ext[2] + u01_53(c[2], c[3]) * (ext[3] - ext[2]);
-        if (env_contains(qx, qy, walls, n_poly, hole0, n_hole)) { px = D(qx); py = D(qy); break; }
-      }
-    }
-  } else if (!((px.v > ext[0]) && (px.v < ext[1]) && (py.v > ext[2]) && (py.v < ext[3]))) {
-    if (periodic) {                                     // pos % extent (Environment.py:877-879)
-      px = D(np_mod(px.v, ext[1]));
-      py = D(np_mod(py.v, ext[3]));
-    } else {
-      px = D(fmin(fmax(px.v, ext[0] + 0.01), ext[1] - 0.01));
-      py = D(fmin(fmax(py.v, ext[2] + 0.01), ext[3] - 0.01));
-    }
+  {
+    // (the reference re-draws from np.random; a Philox stream keyed like the zero-displacement fall-back here)
+    const long long k1 = __double_as_longlong(fallback_n1), k2 = __double_as_longlong(fallback_n2);
+    apply_boundary(px, py, ext, walls, periodic, polygon, n_poly, hole0, n_hole, [&](uint32_t t, double& u1, double& u2) {
+      uint32_t c[4] = {(uint32_t)k2, (uint32_t)(k2 >> 32), 0x52534d50u + t, RIAB_STREAM_MEASURE << 24};
+      philox4x32_10(c, (uint32_t)k1, (uint32_t)(k1 >> 32));
+      u1 = u01_53(c[0], c[1]);
+      u2 = u01_53(c[2], c[3]);
+    });
   }
   D stx, sty, mvx, mvy;
   step_displacement(px, py, ppx, ppy, periodic, scale, stx, sty);
