@@ -434,7 +434,8 @@ typedef struct {
 typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RIAB_CELLS_OVC = 3,
                RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7,
                RIAB_CELLS_TD = 8 /* riab_td_cells: a FeedForwardLayer learning by TD (ValueNeuron, SuccessorFeatures) */,
-               RIAB_CELLS_PPPC = 9 /* riab_pppc_cells: PhasePrecessingPlaceCells */
+               RIAB_CELLS_PPPC = 9 /* riab_pppc_cells: PhasePrecessingPlaceCells */,
+               RIAB_CELLS_PWN = 10 /* riab_pwn_cells: PlaneWaveNeurons */
 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
@@ -618,6 +619,28 @@ typedef struct {
 int riab_pppc_rates(const double* pos_dev, const double* velocity_dev, int64_t n_pos, const riab_env* env,
                     const riab_pppc_cells* cells, float* out_dev, int64_t ld_out, void* stream);
 
+/* ---------------------------------------------------- PlaneWaveNeurons (RIAB_CELLS_PWN)
+ * contribs/PlaneWaveNeurons.py:63-91: phi_i = (2 pi / wavescale_i) ((phase_offset_i - pos) . w_i),
+ *   rate_i = 0.5 (cos phi_i + 1) (max_fr - min_fr) + min_fr   (w as stored: not renormalised)
+ * Rates lie between min_fr and max_fr; riab_run takes a lone PlaneWaveNeurons population as one launch like Place / Grid. */
+typedef struct {
+  int32_t n_cells;
+  int32_t n_pad;           /* filled by riab_pwn_pack */
+  float min_fr, max_fr;
+  const float* packed_dev; /* riab_pwn_pack output, 16-byte aligned */
+  int32_t phase_turns;     /* filled by riab_pwn_pack: 1 = wave vectors as float32 hi / lo pairs and phases in turns, for
+                              the compensated phase of large |k| r_max (riab_pwn.cuh); 0 = radians */
+  int32_t reserved;
+} riab_pwn_cells;
+int64_t riab_pwn_pack_floats(int32_t n_cells);
+/* phase_offsets_host / w_host (N,2), wavescales_host (N) f64; extent the environment's.  phase_form: -1 chooses (turns when
+ * max |2 pi w / wavescale| times the box's half-diagonal exceeds 40), 0 forces radians, 1 forces turns. */
+int riab_pwn_pack(const double* phase_offsets_host, const double* w_host, const double* wavescales_host, int32_t n_cells,
+                  const double* extent, int32_t phase_form, riab_pwn_cells* meta_out, float* out_host);
+/* PlaneWaveNeurons.get_state at pos_dev (n_pos,2) f64 -> out_dev (n_pos, ld_out) f32 */
+int riab_pwn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_pwn_cells* cells,
+                   float* out_dev, int64_t ld_out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
@@ -629,7 +652,8 @@ int riab_pppc_rates(const double* pos_dev, const double* velocity_dev, int64_t n
 typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
-                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* / riab_pppc_cells* */
+                                   riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* / riab_pppc_cells* /
+                                   riab_pwn_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */
@@ -650,7 +674,7 @@ int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_p
 
 /* riab_run following a motion source (src == NULL or RIAB_MOTION_RANDOM: riab_run).  RIAB_MOTION_IMPORTED: step s
  * reads the trajectory at (t + dt + ... + dt) % t_max, the clock advanced by `t += dt` like Agent.update.  A single
- * Place / Grid population runs as one launch where riab_run's would; otherwise every step is the motion kernel followed
+ * Place / Grid / PlaneWave population runs as one launch where riab_run's would; otherwise every step is the motion kernel followed
  * by the populations' rates.  RIAB_MOTION_FORCED is refused: a forced position belongs to one step. */
 int riab_run_src(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
                  const riab_motion_source* src, const riab_population* pops, int32_t n_pops,

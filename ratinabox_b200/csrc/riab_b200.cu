@@ -5,7 +5,8 @@
 //   k_agent_update_src  Agent.update from an imported trajectory / forced positions, one agent per thread (float64)
 //   k_traj_build        not-a-knot spline of imported trajectories, one thread per (trajectory, axis) column
 //   k_step<P,MODE,..>   persistent warp-specialised step kernel for PlaceCells / GridCells / ObjectVectorCells /
-//                       head direction, velocity and speed cells / AgentVectorCells / PhasePrecessingPlaceCells:
+//                       head direction, velocity and speed cells / AgentVectorCells / PhasePrecessingPlaceCells /
+//                       PlaneWaveNeurons:
 //                       producer warps run Agent.update (float64) and publish per-agent float32
 //                       records through an mbarrier ring; consumer warps keep 4 cells per thread
 //                       in registers and stream float4 rate rows (+ OU noise, + bit-packed spikes)
@@ -33,6 +34,7 @@
 #include "riab_motion.cuh"
 #include "riab_place.cuh"
 #include "riab_pppc.cuh"
+#include "riab_pwn.cuh"
 #include "riab_rsn.cuh"
 #include "riab_traj.cuh"
 #include "riab_td.cuh"
@@ -92,7 +94,7 @@ struct OutK {
   float thin_c1, thin_c0;   // accept <=> fma(float(20-bit uniform), c1, c0) < rate;  c1 = 2^-20 bound, c0 = 2^-21 bound
 };
 
-// MODE 3 of k_step: the whole riab_run loop of a single Place / Grid population in ONE launch.  Agents are independent and
+// MODE 3 of k_step: the whole riab_run loop of a single Place / Grid / PlaneWave population in ONE launch.  Agents are independent and
 // the tile -> CTA assignment is static, so a CTA can run all n_steps for its own agents with no grid-wide synchronisation:
 // the producers keep advancing their tiles into the next step while the consumers still write the rates of this one, and
 // the per-launch ramp (wall staging, cell registers, first records) and tail are paid once per run instead of once per step.
@@ -541,6 +543,35 @@ struct PppcPolicy {
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const& c) { return c.wall0; }
+};
+
+// PlaneWaveNeurons (riab_pwn.cuh): one cosine per rate.  The phase form (radians, or compensated turns) is a uniform
+// run-time branch of one kernel, so the population costs 15 k_step instantiations, not 30.
+struct PwnPolicy {
+  using Const = PwnConst;
+  using Regs = PwnCellRegs;
+  static constexpr int REC = 4;
+  // Chosen with scripts/bench_pwn.py (65 536 agents x 1 024 cells, whole run, compensated phase; H100 80GB HBM3, 700 W):
+  // spikes on, the dense stream in StepCfg<4> ran 119.6 us / step against 134.1 with the thinned stream and 135.3 with
+  // LIGHT's dense StepCfg<12>, so THIN = false and LIGHT = false; without spikes LIGHT's StepCfg<8> would save 3 us
+  // (90.3 against 93.4), less than it costs with spikes, which the reference records by default.
+  static constexpr bool LIGHT = false;
+  static constexpr bool THIN = false;
+  static constexpr bool POSITIONAL = true;
+  static __device__ __forceinline__ void given_dir(const Const&, long long, double&, double&) {}
+  static __device__ __forceinline__ void prepare(double*, const double*, const Const&) {}
+  static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double, double, double, double, double, double,
+                                                const double*, const double*, const Const&, const EnvK& env) {
+    pwn_agent_record(rec, px, py, env.cxm, env.cym);
+  }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { pwn_load_cells(r, c, cell0); }
+  template <bool DEFER, int EXP = -1>
+  static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int, const float* rec,
+                                                uint32_t, bool&) {
+    pwn_rates4(o, r, c, rec);
+  }
+  static __device__ __forceinline__ int expanded(const Const&) { return 0; }
+  static __device__ __forceinline__ int wall0(const Const&) { return 0; }
 };
 
 // ---------------------------------------------------------------------------
@@ -1839,6 +1870,21 @@ int make_pppc(const riab_pppc_cells* pc, const EnvK& env, const double* vel, Ppp
   return 0;
 }
 
+// PlaneWaveNeurons: rate = 0.5 (cos phi + 1) span + min_fr = As cos phi + Bs (PlaneWaveNeurons.py:85-89)
+int make_pwn(const riab_pwn_cells* pw, PwnConst& c) {
+  if (pw == nullptr || pw->packed_dev == nullptr) return fail(RIAB_ERR_INVALID, "plane wave neurons / packed_dev NULL");
+  if (pw->n_cells <= 0 || pw->n_pad != (pw->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD)
+    return fail(RIAB_ERR_INVALID, "plane wave neurons: n_cells %d / n_pad %d (pack with riab_pwn_pack)", pw->n_cells, pw->n_pad);
+  if (((uintptr_t)pw->packed_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "plane wave neurons: packed_dev must be 16-byte aligned");
+  memset(&c, 0, sizeof(c));
+  c.n_cells = pw->n_cells; c.n_pad = pw->n_pad;
+  const double half = 0.5 * ((double)pw->max_fr - (double)pw->min_fr);
+  c.As = (float)half; c.Bs = (float)(half + (double)pw->min_fr);
+  c.packed = pw->packed_dev;
+  c.turns = pw->phase_turns ? 1 : 0;
+  return 0;
+}
+
 int g_num_sms = 0;
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
@@ -2340,7 +2386,7 @@ struct Pop {
   int kind = -1, n_cells = 0;
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
-  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc; PppcConst pppc;
+  PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc; PppcConst pppc; PwnConst pwn;
   const riab_bvc_cells* bvc = nullptr; float* bvc_scratch = nullptr; int32_t* first_wall = nullptr;
   const riab_ffl_cells* ffl = nullptr;
   const riab_td_cells* td = nullptr;    // RIAB_CELLS_TD: its layer is `ffl`
@@ -2388,6 +2434,11 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   } else if (kind == RIAB_CELLS_PPPC) {
     rc = make_pppc((const riab_pppc_cells*)cells, ek, ag.velocity, d.pppc);
     d.n_cells = ((const riab_pppc_cells*)cells)->place.n_cells;
+  } else if (kind == RIAB_CELLS_PWN) {
+    const riab_pwn_cells* pw = (const riab_pwn_cells*)cells;
+    rc = make_pwn(pw, d.pwn);
+    d.n_cells = pw->n_cells;
+    d.bound = fmaxf(pw->min_fr, pw->max_fr);
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
@@ -2415,6 +2466,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
   if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, ag.n_agents, s);
   if (d.kind == RIAB_CELLS_PPPC) return launch_pppc<MODE>(ek, ag, mp, io, d.pppc, d.out, pos_in, ag.n_agents, s);
+  if (d.kind == RIAB_CELLS_PWN) return launch_tile<PwnPolicy, MODE>(ek, ag, mp, io, d.pwn, d.out, pos_in, ag.n_agents, s);
   if constexpr (MODE == 0) {
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
@@ -2543,8 +2595,8 @@ int whole_run_applies(const EnvK& ek, const riab_agents& ag, const riab_motion_p
       (src == nullptr && (io.xi != nullptr || io.collision_mask || io.first_hit || io.n_iters)))
     return 0;
   const riab_population& pp = pops[0];
-  if ((pp.kind != RIAB_CELLS_PLACE && pp.kind != RIAB_CELLS_GRID) || pp.rates_ring == nullptr || pp.ring_rows <= 0 ||
-      pp.noise.noise_std != 0.f)
+  if ((pp.kind != RIAB_CELLS_PLACE && pp.kind != RIAB_CELLS_GRID && pp.kind != RIAB_CELLS_PWN) || pp.rates_ring == nullptr ||
+      pp.ring_rows <= 0 || pp.noise.noise_std != 0.f)
     return 0;
   riab_rates_out ro = pp.out;
   ro.rates_row = pp.rates_ring; ro.spikes_row = pp.spikes_ring;
@@ -2555,7 +2607,7 @@ int whole_run_applies(const EnvK& ek, const riab_agents& ag, const riab_motion_p
   const OutK& ok = d.out;
   const long long A = ag.n_agents;
   const bool place = pp.kind == RIAB_CELLS_PLACE;
-  const int ct = (place ? d.place.n_pad : d.grid.n_pad) / 4;
+  const int ct = (place ? d.place.n_pad : pp.kind == RIAB_CELLS_PWN ? d.pwn.n_pad : d.grid.n_pad) / 4;
   const bool rows_ok = ((A * ok.ld) % 4 == 0) && ((A * ok.spike_ld) % 4 == 0);        // every ring row stays 16-byte aligned
   const bool lean = ok.vec_ok && rows_ok && (d.n_cells % 4 == 0) && ct <= RW * 32 &&
                     (ok.spikes == nullptr || (ag.id_offset & 1) == 0) &&
@@ -2642,6 +2694,9 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
     if (pp.kind == RIAB_CELLS_PLACE)
       return src ? launch_place<4>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run)
                  : launch_place<3>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run);
+    if (pp.kind == RIAB_CELLS_PWN)
+      return src ? launch_tile<PwnPolicy, 4>(ek, *agents, *prm, io0, d.pwn, d.out, nullptr, A, s, &run)
+                 : launch_tile<PwnPolicy, 3>(ek, *agents, *prm, io0, d.pwn, d.out, nullptr, A, s, &run);
     if (d.grid.turns)
       return src ? launch_tile<GridPolicy<1>, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
                  : launch_tile<GridPolicy<1>, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
@@ -3298,6 +3353,53 @@ int riab_grid_pack(const double* gridscales, const double* phase_offsets, const 
 int riab_grid_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_grid_cells* gc,
                     float* out_dev, int64_t ld_out, void* stream) {
   return rates_at(RIAB_CELLS_GRID, gc, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream);
+}
+
+// ----------------------------------------------------------- PlaneWaveNeurons
+int64_t riab_pwn_pack_floats(int32_t n_cells) { return (int64_t)place_n_pad(n_cells) * 5; }
+
+int riab_pwn_pack(const double* phase_offsets, const double* w, const double* wavescales, int32_t n, const double* extent,
+                  int32_t phase_form, riab_pwn_cells* meta, float* out) {
+  if (!phase_offsets || !w || !wavescales || !extent || !meta || !out || n <= 0 || phase_form < -1 || phase_form > 1)
+    return fail(RIAB_ERR_INVALID, "riab_pwn_pack: bad argument");
+  const int np = place_n_pad(n);
+  const double cxm = 0.5 * (extent[0] + extent[1]), cym = 0.5 * (extent[2] + extent[3]);
+  const double rmax = 0.5 * hypot(extent[1] - extent[0], extent[3] - extent[2]);
+  for (int64_t i = 0; i < (int64_t)np * 5; ++i) out[i] = 0.f;
+  // The radian form's rate error grows like 1.2e-7 |2 pi k| r_max of the span (r_max: the box's half-diagonal), as for
+  // GridCells: past |2 pi k| r_max = 40 (4.8e-6) the block holds turns for the compensated phase (riab_pwn.cuh).
+  double kr = 0.0;
+  for (int i = 0; i < n; ++i) {
+    const double kx = w[2 * i] / wavescales[i], ky = w[2 * i + 1] / wavescales[i];
+    if (!(std::isfinite(kx) && std::isfinite(ky) && std::isfinite(phase_offsets[2 * i]) && std::isfinite(phase_offsets[2 * i + 1])))
+      return fail(RIAB_ERR_INVALID, "riab_pwn_pack: cell %d: w / wavescale or phase offset not finite", i);
+    kr = fmax(kr, 2.0 * M_PI * hypot(kx, ky) * rmax);
+  }
+  const int turns = phase_form >= 0 ? phase_form : (kr > 40.0 ? 1 : 0);
+  for (int i = 0; i < n; ++i) {
+    const double kx = w[2 * i] / wavescales[i], ky = w[2 * i + 1] / wavescales[i];
+    const double ph = remainder(kx * (phase_offsets[2 * i] - cxm) + ky * (phase_offsets[2 * i + 1] - cym), 1.0);   // turns
+    if (turns) {
+      const float hx = (float)kx, hy = (float)ky;
+      out[(size_t)0 * np + i] = hx;
+      out[(size_t)1 * np + i] = hy;
+      out[(size_t)2 * np + i] = (float)(kx - (double)hx);
+      out[(size_t)3 * np + i] = (float)(ky - (double)hy);
+      out[(size_t)4 * np + i] = (float)ph;
+    } else {
+      out[(size_t)0 * np + i] = (float)(2.0 * M_PI * kx);
+      out[(size_t)1 * np + i] = (float)(2.0 * M_PI * ky);
+      out[(size_t)4 * np + i] = (float)(2.0 * M_PI * ph);
+    }
+  }
+  meta->n_pad = np;
+  meta->phase_turns = turns;
+  return 0;
+}
+
+int riab_pwn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_pwn_cells* cells, float* out_dev,
+                   int64_t ld_out, void* stream) {
+  return rates_at(RIAB_CELLS_PWN, cells, pos_dev, n_pos, env, nullptr, nullptr, nullptr, out_dev, ld_out, stream);
 }
 
 // ------------------------------------------------------------------------ BVC
