@@ -435,7 +435,8 @@ typedef enum { RIAB_CELLS_PLACE = 0, RIAB_CELLS_GRID = 1, RIAB_CELLS_BVC = 2, RI
                RIAB_CELLS_FFL = 4, RIAB_CELLS_RSN = 5, RIAB_CELLS_KIN = 6, RIAB_CELLS_AVC = 7,
                RIAB_CELLS_TD = 8 /* riab_td_cells: a FeedForwardLayer learning by TD (ValueNeuron, SuccessorFeatures) */,
                RIAB_CELLS_PPPC = 9 /* riab_pppc_cells: PhasePrecessingPlaceCells */,
-               RIAB_CELLS_PWN = 10 /* riab_pwn_cells: PlaneWaveNeurons */
+               RIAB_CELLS_PWN = 10 /* riab_pwn_cells: PlaneWaveNeurons */,
+               RIAB_CELLS_NNN = 11 /* riab_nnn_cells: NeuralNetworkNeurons */
 } riab_cells_kind;
 typedef struct {
   float* rates_row;        /* (A, ld) f32: firing rates of this step (doubles as the history row) */
@@ -641,11 +642,50 @@ int riab_pwn_pack(const double* phase_offsets_host, const double* w_host, const 
 int riab_pwn_rates(const double* pos_dev, int64_t n_pos, const riab_env* env, const riab_pwn_cells* cells,
                    float* out_dev, int64_t ld_out, void* stream);
 
+/* ------------------------------------------------ NeuralNetworkNeurons (RIAB_CELLS_NNN)
+ * contribs/NeuralNetworkNeurons.py:74-104 for a module that is a chain of Linear layers and elementwise activations:
+ *   h_0 = [I_0 | I_1 | ...] (the inputs' rates, concatenated in input order), h_l = act_l(W_l h_{l-1} + b_l), rates = h_L.
+ * One launch per evaluation (riab_nnn.cuh, k_nnn): layer 1 is the FeedForwardLayer's error-compensated TF32 wgmma GEMM
+ * over the gathered input rows; the hidden activations stay in shared memory and the later layers run in float32 FMA.
+ * Limits of the fused kernel: 1..RIAB_NNN_MAX_LAYERS Linear layers, hidden widths (widths[1 .. n_layers-1]) of at most
+ * RIAB_NNN_MAX_HIDDEN, at most RIAB_FFL_MAX_INPUTS input populations; the input count (widths[0]) and the output width
+ * are unbounded.  Rows whose position x is NaN get zeros, then OU noise and spikes as for every population.  riab_run
+ * treats the kind like a FeedForwardLayer (plain schedule, input rows by registration-order lag). */
+#define RIAB_NNN_MAX_LAYERS 8
+#define RIAB_NNN_MAX_HIDDEN 256
+typedef enum { RIAB_NNN_IDENTITY = 0, RIAB_NNN_RELU = 1, RIAB_NNN_SIGMOID = 2 /* 1 / (1 + exp(-x)) */, RIAB_NNN_TANH = 3
+} riab_nnn_activation;
+typedef struct {
+  int32_t n_cells;                            /* filled by riab_nnn_pack: widths[n_layers] */
+  int32_t n_layers;                           /* Linear layers.  0: the rates were computed by the caller (a module the
+                                                 kernel does not run) and sit in inputs[0].rows_dev (n_rows, ld, n_in =
+                                                 n_cells): the library only masks NaN rows, adds noise and draws spikes */
+  int32_t n_inputs;
+  int32_t widths[RIAB_NNN_MAX_LAYERS + 1];    /* widths[0] = the sum of inputs[i].n_in, widths[l] = layer l's outputs */
+  int32_t act[RIAB_NNN_MAX_LAYERS];           /* riab_nnn_activation applied after Linear layer l + 1 */
+  const float* packed_dev;                    /* riab_nnn_pack block, 16-byte aligned */
+  riab_ffl_input inputs[RIAB_FFL_MAX_INPUTS]; /* n_in, rows_dev, ld, population, lag as for a FeedForwardLayer; w_dev is
+                                                 unused (layer 1's weights are in packed_dev) */
+} riab_nnn_cells;
+/* Floats of the packed block of `meta` (n_layers, widths, n_inputs, inputs[i].n_in set):
+ *   for each input i, riab_ffl_pack of W_1's columns of that input (riab_ffl_pack_floats(widths[1], n_in_i) floats);
+ *   b_1 (widths[1] rounded up to 8); then per layer l >= 2, W_l^T (widths[l-1], widths[l] rounded up to 8) and b_l. */
+int64_t riab_nnn_pack_floats(const riab_nnn_cells* meta);
+/* params_host: per Linear layer l = 1..n_layers, W_l (widths[l], widths[l-1]) f64 row-major then b_l (widths[l]) (zeros
+ * for a Linear without bias).  meta in: n_layers, widths, act, n_inputs, inputs[i].n_in; out: n_cells, inputs[i].k_pad.
+ * Refuses what the fused kernel does not run (the limits above). */
+int riab_nnn_pack(const double* params_host, riab_nnn_cells* meta, float* out_host);
+/* The network over n_rows input rows (cells->inputs[i].rows_dev) -> out->rates_row (n_rows, ld), then OU noise and spikes
+ * (noise NULL: rates only); pos_dev (n_rows, 2) f64 or NULL: rows whose x is NaN get zeros.  With RIAB_CELLS_NNN,
+ * riab_neurons_update / riab_step_fused call this for the agents' rows and positions. */
+int riab_nnn_rates(const riab_nnn_cells* cells, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
+                   const riab_rates_out* out, void* stream);
+
 /* ------------------------------------------------------------- multi-step run
  * `for _ in range(n_steps): Ag.update(); [Ns.update() for Ns in Ag.Neurons]`
  * (tests/test_advanced.py:21-23) without returning to the host between steps.
  * Population 0 is fused with the motion kernel, the others use riab_neurons_update; FeedForwardLayers
- * (RIAB_CELLS_FFL, and RIAB_CELLS_TD with its trace pass) run after every other population of the step, in index order,
+ * (RIAB_CELLS_FFL, RIAB_CELLS_TD with its trace pass, and RIAB_CELLS_NNN) run after every other population of the step, in index order,
  * reading ring rows (next + s - lag) of their inputs, and an Agent with one keeps this unskewed schedule.  A TD layer's
  * self-recurrent input reads its fr_prev.  riab_run never calls riab_td_learn.
  * History rows go to device rings: row (next + s) % rows for step s. */
@@ -653,7 +693,7 @@ typedef struct {
   int32_t kind;                 /* riab_cells_kind */
   const void* cells;            /* riab_place_cells* / riab_grid_cells* / riab_bvc_cells* / riab_ovc_cells* / riab_ffl_cells* /
                                    riab_rsn_cells* / riab_kin_cells* / riab_avc_cells* / riab_td_cells* / riab_pppc_cells* /
-                                   riab_pwn_cells* */
+                                   riab_pwn_cells* / riab_nnn_cells* */
   riab_neuron_noise noise;      /* seed/step base; step is advanced per step */
   riab_rates_out out;           /* ld, noise_state, bvc_scratch; rates_row/spikes_row are set from the rings */
   float* rates_ring;            /* (rows, A, ld) f32 */

@@ -597,6 +597,8 @@ class Agent:
         if kwargs.get("forced_next_position", None) is not None:
             raise NotImplementedError("run() cannot take forced_next_position: a forced position belongs to one step; "
                                       "step with update(forced_next_position=...)")
+        for ns in self.Neurons:
+            ns._check_run()
         # stage everything exactly like one update() would, then hand the loop to C
         self._staging_only = True
         try:

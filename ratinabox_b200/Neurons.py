@@ -103,6 +103,9 @@ class Neurons:
         """The struct Agent.run hands to riab_run."""
         return self._cells()
 
+    def _check_run(self):
+        """Raise if riab_run cannot run this population (Agent.run calls it before it stages anything)."""
+
     def _rates_from_positions(self, pos_dev, n_pos, out):
         raise NotImplementedError
 

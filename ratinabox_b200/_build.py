@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("RIAB_LIB", os.path.join(HERE, "libriab_b200.so"))
-SOURCES = ["riab_b200.cu"]
+SOURCES = ["riab_b200.cu", "riab_nnn.cu"]
 HEADERS = None  # every csrc/*.cuh + include/riab_b200.h (see _headers)
 
 NVCC_FLAGS = [

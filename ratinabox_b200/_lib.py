@@ -169,6 +169,16 @@ class PwnCells(C.Structure):
                 ("packed_dev", C.c_void_p), ("phase_turns", C.c_int32), ("reserved", C.c_int32)]
 
 
+NNN_MAX_LAYERS, NNN_MAX_HIDDEN = 8, 256
+NNN_ACTIVATIONS = {"identity": 0, "relu": 1, "sigmoid": 2, "tanh": 3}   # riab_nnn_activation
+
+
+class NnnCells(C.Structure):
+    _fields_ = [("n_cells", C.c_int32), ("n_layers", C.c_int32), ("n_inputs", C.c_int32),
+                ("widths", C.c_int32 * (NNN_MAX_LAYERS + 1)), ("act", C.c_int32 * NNN_MAX_LAYERS),
+                ("packed_dev", C.c_void_p), ("inputs", FflInput * FFL_MAX_INPUTS)]
+
+
 class HistoryView(C.Structure):
     _fields_ = [("agent_ring", C.c_void_p), ("agent_ring_rows", C.c_int32), ("agent_row0", C.c_int32),
                 ("rates_ring", C.c_void_p), ("rates_ring_rows", C.c_int32), ("rates_row0", C.c_int32),
@@ -200,7 +210,7 @@ PC_DESCRIPTIONS = {"gaussian": 0, "gaussian_threshold": 1, "diff_of_gaussians": 
 WALL_GEOMETRIES = {"euclidean": 0, "line_of_sight": 1, "geodesic": 2}
 GC_DESCRIPTIONS = {"rectified_cosines": 0, "shifted_cosines": 1}
 (CELLS_PLACE, CELLS_GRID, CELLS_BVC, CELLS_OVC, CELLS_FFL, CELLS_RSN, CELLS_KIN, CELLS_AVC, CELLS_TD, CELLS_PPPC,
- CELLS_PWN) = range(11)
+ CELLS_PWN, CELLS_NNN) = range(12)
 KIN_HEAD_DIRECTION, KIN_VELOCITY, KIN_SPEED = 0, 1, 2                # riab_kin_variant
 PLACE_MAX_WI = 8                                              # inner walls of the line-of-sight / geodesic kernels
 ACTIVATIONS = {"linear": 0, "sigmoid": 1, "relu": 2, "tanh": 3, "retanh": 4, "softmax": 5}   # riab_activation
@@ -266,6 +276,10 @@ SYMBOLS = {
     "riab_pwn_pack": (C.c_int, [c_double_p, c_double_p, c_double_p, C.c_int32, c_double_p, C.c_int32, C.POINTER(PwnCells),
                                 c_float_p]),
     "riab_pwn_rates": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(Env), C.POINTER(PwnCells), C.c_void_p, C.c_int64, C.c_void_p]),
+    "riab_nnn_pack_floats": (C.c_int64, [C.POINTER(NnnCells)]),
+    "riab_nnn_pack": (C.c_int, [c_double_p, C.POINTER(NnnCells), c_float_p]),
+    "riab_nnn_rates": (C.c_int, [C.POINTER(NnnCells), C.c_int64, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut),
+                                 C.c_void_p]),
     "riab_step_fused": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.POINTER(MotionParams), C.POINTER(StepIO),
                                   C.c_int32, C.c_void_p, C.POINTER(NeuronNoise), C.POINTER(RatesOut), C.c_void_p]),
     "riab_neurons_update": (C.c_int, [C.POINTER(Agents), C.POINTER(Env), C.c_int32, C.c_void_p, C.POINTER(NeuronNoise),

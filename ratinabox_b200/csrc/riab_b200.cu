@@ -13,6 +13,7 @@
 //   k_bvc_rays<TABLE>   BVC phase A (float64 rays)
 //   k_bvc_integrate     BVC phase B (float32 angular integral, TMA-staged tables)
 //   k_td_*              TD learning of ValueNeuron / SuccessorFeatures (riab_td.cuh)
+//   k_nnn<BN>           NeuralNetworkNeurons: a Linear / activation chain over the input rows, one launch (riab_nnn.cu)
 //   k_theta_seq         ThetaSequenceAgent sweep positions over a lead Agent's batch, one agent per thread (float64)
 //   k_subagent          DumbAgent / ShiftAgent / ReplayAgent positions over a lead Agent's batch, one agent per thread (float64)
 #include <algorithm>
@@ -32,6 +33,7 @@
 #include "riab_grid.cuh"
 #include "riab_kin.cuh"
 #include "riab_motion.cuh"
+#include "riab_nnn.cuh"
 #include "riab_place.cuh"
 #include "riab_pppc.cuh"
 #include "riab_pwn.cuh"
@@ -2211,6 +2213,90 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
 }
 
 // ---------------------------------------------------------------------------
+// NeuralNetworkNeurons (riab_nnn.cuh).  Layer 1's W_hi | W_lo block of input i starts after those of inputs 0..i-1.
+long long nnn_w1_offset(const riab_nnn_cells* c, int i) {
+  long long off = 0;
+  for (int j = 0; j < i; ++j) off += 2LL * ((c->widths[1] + 7) / 8 * 8) * ((c->inputs[j].n_in + FFL_BK - 1) / FFL_BK * FFL_BK);
+  return off;
+}
+
+int check_nnn(const riab_nnn_cells* c, long long n_rows) {
+  if (c == nullptr) return fail(RIAB_ERR_INVALID, "nnn cells NULL");
+  if (c->n_cells <= 0) return fail(RIAB_ERR_INVALID, "nnn: n_cells must be > 0");
+  if (c->n_layers < 0 || c->n_layers > RIAB_NNN_MAX_LAYERS)
+    return fail(RIAB_ERR_UNSUPPORTED, "nnn: %d Linear layers (at most %d)", c->n_layers, RIAB_NNN_MAX_LAYERS);
+  if (c->n_inputs < (c->n_layers == 0 ? 1 : 0) || c->n_inputs > RIAB_FFL_MAX_INPUTS)
+    return fail(RIAB_ERR_UNSUPPORTED, "nnn: %d inputs (at most %d)", c->n_inputs, RIAB_FFL_MAX_INPUTS);
+  if (c->n_layers == 0) {
+    const riab_ffl_input& in = c->inputs[0];
+    if (n_rows > 0 && (in.rows_dev == nullptr || in.ld < c->n_cells)) return fail(RIAB_ERR_INVALID, "nnn: bad precomputed rows");
+    return 0;
+  }
+  if (c->packed_dev == nullptr || ((uintptr_t)c->packed_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "nnn: packed_dev NULL or misaligned");
+  int n_in = 0;
+  for (int i = 0; i < c->n_inputs; ++i) {
+    const riab_ffl_input& in = c->inputs[i];
+    if (in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || (in.rows_dev != nullptr && in.ld < in.n_in))
+      return fail(RIAB_ERR_INVALID, "nnn input %d: bad sizes (pack with riab_nnn_pack)", i);
+    if (((uintptr_t)in.rows_dev) % 16 != 0 || (in.ld * 4) % 16 != 0) return fail(RIAB_ERR_INVALID, "NNN inputs need 16-byte aligned rows");
+    n_in += in.n_in;
+  }
+  if (n_in != c->widths[0]) return fail(RIAB_ERR_INVALID, "nnn: inputs give %d rates, widths[0] is %d", n_in, c->widths[0]);
+  for (int l = 1; l <= c->n_layers; ++l) {
+    if (c->widths[l] <= 0) return fail(RIAB_ERR_INVALID, "nnn: width %d of layer %d", c->widths[l], l);
+    if (l < c->n_layers && c->widths[l] > RIAB_NNN_MAX_HIDDEN)
+      return fail(RIAB_ERR_UNSUPPORTED, "nnn: hidden width %d (at most %d)", c->widths[l], RIAB_NNN_MAX_HIDDEN);
+    if (c->act[l - 1] < RIAB_NNN_IDENTITY || c->act[l - 1] > RIAB_NNN_TANH) return fail(RIAB_ERR_INVALID, "nnn: bad activation %d", c->act[l - 1]);
+  }
+  if (c->widths[c->n_layers] != c->n_cells) return fail(RIAB_ERR_INVALID, "nnn: n_cells != the last layer's width");
+  return 0;
+}
+
+// One NeuralNetworkNeurons evaluation over n_rows rows (+ noise / spikes through the k_finish_rows post-pass), checked by
+// check_nnn.  Inputs that were never updated contribute zeros, as for a FeedForwardLayer.
+int launch_nnn(const riab_nnn_cells* c, long long n_rows, const double* pos, const OutK& out, cudaStream_t s) {
+  if (n_rows == 0) return 0;
+  if (c->n_layers == 0) {
+    RIAB_CUDA_OK(nnn_rows_launch(c->inputs[0].rows_dev, c->inputs[0].ld, out.rates, out.ld, c->n_cells, n_rows, pos, s));
+    g_launches++;
+  } else {
+    NnnK k;
+    memset(&k, 0, sizeof(k));
+    int rc;
+    const int h1 = c->widths[1], n_pad = (h1 + 7) / 8 * 8;
+    // N tile of layer 1: 32 columns cover the default MLP's 20 in one chunk; wider first layers take chunks of 64
+    const int bn = h1 <= 32 ? 32 : 64;
+    for (int i = 0; i < c->n_inputs; ++i) {
+      const riab_ffl_input& in = c->inputs[i];
+      const float* w = c->packed_dev + nnn_w1_offset(c, i);
+      if (in.rows_dev == nullptr) continue;
+      const int l = k.n_inputs++;
+      if ((rc = ffl_tmap(&k.in[l], in.rows_dev, in.n_in, n_rows, in.ld, NNN_BM)) ||
+          (rc = ffl_tmap(&k.whi[l], w, in.k_pad, n_pad, in.k_pad, bn)) ||
+          (rc = ffl_tmap(&k.wlo[l], w + (size_t)n_pad * in.k_pad, in.k_pad, n_pad, in.k_pad, bn))) return rc;
+      k.ktiles[l] = in.k_pad / FFL_BK;
+    }
+    k.n_layers = c->n_layers;
+    int hmax = 1;
+    for (int l = 0; l <= c->n_layers; ++l) k.widths[l] = c->widths[l];
+    for (int l = 0; l < c->n_layers; ++l) k.act[l] = c->act[l];
+    for (int l = 1; l < c->n_layers; ++l) hmax = std::max(hmax, c->widths[l]);
+    k.h_ld = hmax | 1;
+    k.bias1 = c->packed_dev + nnn_w1_offset(c, c->n_inputs);
+    k.n_rows = n_rows; k.ld = out.ld; k.rates = out.rates; k.pos = pos;
+    RIAB_CUDA_OK(nnn_launch(k, bn, s));
+    g_launches++;
+  }
+  if (out.noise != nullptr || out.spikes != nullptr) {
+    const int np128 = (c->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
+    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, c->n_cells, np128, n_rows);
+    g_launches++;
+    RIAB_CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------
 // TD learning (riab_td.cuh).  check_td: the TD state of a layer whose riab_ffl_cells part check_ffl already accepted.
 int check_td(const riab_td_cells* t, long long out_ld) {
   if (t == nullptr) return fail(RIAB_ERR_INVALID, "td cells NULL");
@@ -2391,6 +2477,7 @@ struct Pop {
   const riab_ffl_cells* ffl = nullptr;
   const riab_td_cells* td = nullptr;    // RIAB_CELLS_TD: its layer is `ffl`
   const riab_rsn_cells* rsn = nullptr;  // its sample points: `place`
+  const riab_nnn_cells* nnn = nullptr;
 };
 
 int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* out, const riab_neuron_noise* noise,
@@ -2439,17 +2526,21 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
     rc = make_pwn(pw, d.pwn);
     d.n_cells = pw->n_cells;
     d.bound = fmaxf(pw->min_fr, pw->max_fr);
+  } else if (kind == RIAB_CELLS_NNN) {
+    d.nnn = (const riab_nnn_cells*)cells;
+    d.n_cells = d.nnn->n_cells;
   } else {
     return fail(RIAB_ERR_INVALID, "bad cells_kind %d", kind);
   }
   if (rc || (rc = make_out(out, noise, d.n_cells, dt, ag.id_offset, d.out, d.bound))) return rc;
   if (kind == RIAB_CELLS_BVC) return check_bvc(ek, d.bvc, d.bvc_scratch = out->bvc_scratch, ag.n_agents);
   if (kind == RIAB_CELLS_TD) return (rc = check_ffl(d.ffl, d.out, ag.n_agents)) ? rc : check_td(d.td, d.out.ld);
+  if (kind == RIAB_CELLS_NNN) return check_nnn(d.nnn, ag.n_agents);
   return kind == RIAB_CELLS_FFL ? check_ffl(d.ffl, d.out, ag.n_agents) : 0;
 }
 
 // FeedForwardLayer-like kinds: they read other populations' rows and run after them (plan_run)
-bool ffl_like(int kind) { return kind == RIAB_CELLS_FFL || kind == RIAB_CELLS_TD; }
+bool ffl_like(int kind) { return kind == RIAB_CELLS_FFL || kind == RIAB_CELLS_TD || kind == RIAB_CELLS_NNN; }
 
 // One population's kernels for one step.  MODE 0: rates at the agents' positions; 1: the motion step fused in; 2: skewed
 // (rates at the current positions while the motion of the next step runs, riab_run).  BVC, FFL and RSN populations run
@@ -2471,6 +2562,7 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
     if (d.kind == RIAB_CELLS_BVC)
       return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
     if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, ag.n_agents, d.out, s);
+    if (d.kind == RIAB_CELLS_NNN) return launch_nnn(d.nnn, ag.n_agents, ag.pos, d.out, s);
     const int rc = launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
     return (rc || d.kind != RIAB_CELLS_TD) ? rc : launch_td_trace(d.td, ag.n_agents, d.out.rates, s);
   } else {
@@ -2480,11 +2572,11 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
 
 // The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), one_hot (an
 // arg-min across cells), BVC (the latency-bound ray kernel wants all its CTAs in ONE wave: the 128-register motion code
-// would halve its occupancy), FeedForwardLayers (they read other populations' rows, not the positions) and
-// RandomSpatialNeurons (a GEMM kernel without motion warps).
+// would halve its occupancy), FeedForwardLayers and NeuralNetworkNeurons (they read other populations' rows, not the
+// positions) and RandomSpatialNeurons (a GEMM kernel without motion warps).
 bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
   return io.collision_mask || io.first_hit || io.n_iters || d.kind == RIAB_CELLS_BVC || d.kind == RIAB_CELLS_FFL ||
-         d.kind == RIAB_CELLS_TD || d.kind == RIAB_CELLS_RSN ||
+         d.kind == RIAB_CELLS_TD || d.kind == RIAB_CELLS_RSN || d.kind == RIAB_CELLS_NNN ||
          (d.kind == RIAB_CELLS_PLACE && d.place.desc == RIAB_PC_ONE_HOT);
 }
 
@@ -2743,6 +2835,7 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
       nz.step = pp.noise.step + (uint64_t)st; nz.dt = prm->dt;
       riab_td_cells tc;                             // an FFL population uses tc.ffl only
       riab_ffl_cells& fc = tc.ffl;
+      riab_nnn_cells nc;
       riab_pppc_cells ppc;
       const void* cells = pp.cells;
       if (pp.kind == RIAB_CELLS_PPPC && pp.cells != nullptr) {
@@ -2753,16 +2846,27 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
       if (ffl_like(pp.kind)) {
         // inputs registered before the layer give this step's ring row, the others (the layer itself included) the
         // previous step's: before the first step, the row the caller passed
-        if (pp.kind == RIAB_CELLS_TD) {
-          if (pp.cells == nullptr) return fail(RIAB_ERR_INVALID, "population %d: cells NULL", p);
-          tc = *(const riab_td_cells*)pp.cells;
-          cells = &tc;
+        int n_inputs;
+        riab_ffl_input* inputs;
+        if (pp.cells == nullptr) return fail(RIAB_ERR_INVALID, "population %d: cells NULL", p);
+        if (pp.kind == RIAB_CELLS_NNN) {
+          nc = *(const riab_nnn_cells*)pp.cells;
+          if (nc.n_layers == 0)
+            return fail(RIAB_ERR_UNSUPPORTED, "population %d: a NeuralNetworkNeurons module the kernel does not run", p);
+          cells = &nc;
+          n_inputs = nc.n_inputs; inputs = nc.inputs;
         } else {
-          fc = *(const riab_ffl_cells*)pp.cells;
-          cells = &fc;
+          if (pp.kind == RIAB_CELLS_TD) {
+            tc = *(const riab_td_cells*)pp.cells;
+            cells = &tc;
+          } else {
+            fc = *(const riab_ffl_cells*)pp.cells;
+            cells = &fc;
+          }
+          n_inputs = fc.n_inputs; inputs = fc.inputs;
         }
-        for (int i = 0; i < fc.n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
-          riab_ffl_input& in = fc.inputs[i];
+        for (int i = 0; i < n_inputs && i < RIAB_FFL_MAX_INPUTS; ++i) {
+          riab_ffl_input& in = inputs[i];
           if (in.population < 0 || in.population >= n_pops || (in.lag == 0) != (in.population < p) || in.lag < 0 || in.lag > 1)
             return fail(RIAB_ERR_INVALID, "population %d: FeedForwardLayer input %d (population %d, lag %d) out of order", p, i,
                         in.population, in.lag);
@@ -3649,6 +3753,85 @@ int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_
   if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
       (rc = check_ffl(ffl, ok, n_rows))) return rc;
   return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------ NeuralNetworkNeurons
+int64_t riab_nnn_pack_floats(const riab_nnn_cells* meta) {
+  if (meta == nullptr || meta->n_layers < 1 || meta->n_layers > RIAB_NNN_MAX_LAYERS || meta->n_inputs < 1 ||
+      meta->n_inputs > RIAB_FFL_MAX_INPUTS)
+    return -1;
+  int64_t n = 0;
+  for (int i = 0; i < meta->n_inputs; ++i) n += riab_ffl_pack_floats(meta->widths[1], meta->inputs[i].n_in);
+  n += ffl_n_pad(meta->widths[1]);
+  for (int l = 2; l <= meta->n_layers; ++l) n += (int64_t)(meta->widths[l - 1] + 1) * ffl_n_pad(meta->widths[l]);
+  return n;
+}
+
+int riab_nnn_pack(const double* params, riab_nnn_cells* meta, float* out) {
+  if (params == nullptr || meta == nullptr || out == nullptr) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: bad argument");
+  const int L = meta->n_layers;
+  if (L < 1 || L > RIAB_NNN_MAX_LAYERS)
+    return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: %d Linear layers (1 to %d)", L, RIAB_NNN_MAX_LAYERS);
+  if (meta->n_inputs < 1 || meta->n_inputs > RIAB_FFL_MAX_INPUTS)
+    return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: %d inputs (1 to %d)", meta->n_inputs, RIAB_FFL_MAX_INPUTS);
+  int n_in = 0;
+  for (int i = 0; i < meta->n_inputs; ++i) {
+    if (meta->inputs[i].n_in <= 0) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: input %d has %d rates", i, meta->inputs[i].n_in);
+    n_in += meta->inputs[i].n_in;
+  }
+  if (n_in != meta->widths[0]) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: inputs give %d rates, widths[0] is %d", n_in, meta->widths[0]);
+  for (int l = 1; l <= L; ++l) {
+    if (meta->widths[l] <= 0) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: width %d of layer %d", meta->widths[l], l);
+    if (l < L && meta->widths[l] > RIAB_NNN_MAX_HIDDEN)
+      return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: hidden width %d (at most %d)", meta->widths[l], RIAB_NNN_MAX_HIDDEN);
+    if (meta->act[l - 1] < RIAB_NNN_IDENTITY || meta->act[l - 1] > RIAB_NNN_TANH)
+      return fail(RIAB_ERR_INVALID, "riab_nnn_pack: bad activation %d", meta->act[l - 1]);
+  }
+  // layer 1: W_1's column block of each input through riab_ffl_pack
+  const int h1 = meta->widths[1];
+  const double* p = params;
+  float* o = out;
+  std::vector<double> block;
+  int col0 = 0;
+  for (int i = 0; i < meta->n_inputs; ++i) {
+    const int ni = meta->inputs[i].n_in;
+    block.assign((size_t)h1 * ni, 0.0);
+    for (int r = 0; r < h1; ++r)
+      for (int j = 0; j < ni; ++j) block[(size_t)r * ni + j] = p[(size_t)r * n_in + col0 + j];
+    riab_ffl_input tmp = meta->inputs[i];
+    int rc;
+    if ((rc = riab_ffl_pack(block.data(), h1, ni, &tmp, o))) return rc;
+    meta->inputs[i].k_pad = tmp.k_pad;
+    o += riab_ffl_pack_floats(h1, ni);
+    col0 += ni;
+  }
+  p += (size_t)h1 * n_in;
+  for (int c = 0; c < ffl_n_pad(h1); ++c) o[c] = c < h1 ? (float)p[c] : 0.f;
+  o += ffl_n_pad(h1);
+  p += h1;
+  // layers 2..L: W_l^T (h_in, pad8(h_out)) then b_l
+  for (int l = 2; l <= L; ++l) {
+    const int ni = meta->widths[l - 1], no = meta->widths[l], no8 = ffl_n_pad(no);
+    for (int i = 0; i < ni; ++i)
+      for (int c = 0; c < no8; ++c) o[(size_t)i * no8 + c] = c < no ? (float)p[(size_t)c * ni + i] : 0.f;
+    o += (size_t)ni * no8;
+    p += (size_t)no * ni;
+    for (int c = 0; c < no8; ++c) o[c] = c < no ? (float)p[c] : 0.f;
+    o += no8;
+    p += no;
+  }
+  meta->n_cells = meta->widths[L];
+  return 0;
+}
+
+int riab_nnn_rates(const riab_nnn_cells* cells, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
+                   const riab_rates_out* out, void* stream) {
+  if (cells == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_nnn_rates: bad argument");
+  OutK ok;
+  int rc;
+  if ((rc = make_out(out, noise, cells->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
+      (rc = check_nnn(cells, n_rows))) return rc;
+  return launch_nnn(cells, n_rows, pos_dev, ok, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------ TD learning
