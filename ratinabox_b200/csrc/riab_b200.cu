@@ -1887,7 +1887,26 @@ int make_pwn(const riab_pwn_cells* pw, PwnConst& c) {
   return 0;
 }
 
-int g_num_sms = 0;
+// The current device's SM count, cached per device ordinal (a process may drive several GPUs)
+int num_sms(int& sms) {
+  static int sms_of[64] = {0};
+  int dev = 0;
+  RIAB_CUDA_OK(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return fail(RIAB_ERR_UNSUPPORTED, "device ordinal %d", dev);
+  if (sms_of[dev] == 0) RIAB_CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev], cudaDevAttrMultiProcessorCount, dev));
+  sms = sms_of[dev];
+  return 0;
+}
+
+// The noise / spike post-pass (k_finish_rows) over n_rows rows, when out has either
+int finish_rows(const OutK& out, int n_cells, long long n_rows, cudaStream_t s) {
+  if (out.noise == nullptr && out.spikes == nullptr) return 0;
+  const int np128 = (n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
+  k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, n_cells, np128, n_rows);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
 
 // MODE 0: rates for given positions; 1: motion -> rates (one step); 2: skewed (rates of the current
 // positions, then motion for the NEXT step -- used inside riab_run); 3: the whole run (RunK); 4: the whole run following
@@ -1897,14 +1916,8 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
                 const typename P::Const& pc, const OutK& out_in, const double* pos_in, long long n_rows, cudaStream_t s,
                 const RunK* run_in = nullptr) {
   if (n_rows == 0) return 0;
-  {
-    static int sms_of[64] = {0};                      // SM count per device ordinal (a process may drive several GPUs)
-    int dev = 0;
-    RIAB_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64) return fail(RIAB_ERR_UNSUPPORTED, "device ordinal %d", dev);
-    if (sms_of[dev] == 0) RIAB_CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev], cudaDevAttrMultiProcessorCount, dev));
-    g_num_sms = sms_of[dev];
-  }
+  int sms, rc;
+  if ((rc = num_sms(sms))) return rc;
   const bool spikes = out_in.spikes != nullptr, noise = out_in.noise != nullptr;
   // thinned stream: bounded rates AND a policy for which it measured faster (P::THIN); see the policies
   const bool thin = spikes && !noise && out_in.thin && P::THIN;
@@ -1915,7 +1928,7 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   {
     const int ct = pc.n_pad / 4;                                      // cell-threads of one consumer group
     const int ring = (cfg == 4) ? ring_slots<P, StepCfg<4>>() : (cfg == 8) ? ring_slots<P, StepCfg<8>>() : ring_slots<P, StepCfg<12>>();
-    const long long groups = (ct > 0 && ct <= RW * 32) ? (long long)g_num_sms * lean_groups(ct, ring) : (long long)g_num_sms;
+    const long long groups = (ct > 0 && ct <= RW * 32) ? (long long)sms * lean_groups(ct, ring) : (long long)sms;
     int ta = TA;
     if (n_rows < 4ll * TA * groups) {
       const long long per = (n_rows + groups - 1) / groups;          // agents per group if every group gets one slot
@@ -1932,7 +1945,7 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   memset(&run, 0, sizeof(run));
   if (run_in != nullptr) run = *run_in;
   const long long n_tiles = (n_rows + out.tile_agents - 1) / out.tile_agents;
-  const unsigned grid = (unsigned)(n_tiles < g_num_sms ? n_tiles : g_num_sms);
+  const unsigned grid = (unsigned)(n_tiles < sms ? n_tiles : sms);
   MotionDerived md;
   memset(&md, 0, sizeof(md));
   if (MODE != 0) derive_motion(mp, md);
@@ -1956,23 +1969,20 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   return 0;
 }
 
-template <int MODE, int DESC>
-int launch_place_d(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
-                   const PlaceConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s,
-                   const RunK* run = nullptr) {
-  const int wi = pc.n_inner;
-  if (pc.comp) {
-    if (wi == 0) return launch_tile<PlacePolicy<0, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-    if (wi == 1) return launch_tile<PlacePolicy<1, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-    if (wi == 2) return launch_tile<PlacePolicy<2, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-    if (wi <= 4) return launch_tile<PlacePolicy<4, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-    return launch_tile<PlacePolicy<8, DESC, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+// A Place-like policy (PlacePolicy, PppcPolicy) for pc's compensated-sum switch and inner walls (compile-time bound 0, 1,
+// 2, 4 or 8); called with COMP = false, it first picks COMP from pc.comp
+template <template <int, int, bool> class Pol, int MODE, int DESC, bool COMP = false, class C>
+int launch_walls(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const C& pc,
+                 const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s, const RunK* run) {
+  if constexpr (!COMP) {
+    if (pc.comp) return launch_walls<Pol, MODE, DESC, true>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
   }
-  if (wi == 0) return launch_tile<PlacePolicy<0, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi == 1) return launch_tile<PlacePolicy<1, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi == 2) return launch_tile<PlacePolicy<2, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi <= 4) return launch_tile<PlacePolicy<4, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  return launch_tile<PlacePolicy<8, DESC>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  const int wi = pc.n_inner;
+  if (wi == 0) return launch_tile<Pol<0, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  if (wi == 1) return launch_tile<Pol<1, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  if (wi == 2) return launch_tile<Pol<2, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  if (wi <= 4) return launch_tile<Pol<4, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  return launch_tile<Pol<8, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
 }
 
 int launch_onehot(const EnvK& env, const PlaceConst& pc, const OutK& out, const double* pos, long long n_rows,
@@ -1981,27 +1991,18 @@ int launch_onehot(const EnvK& env, const PlaceConst& pc, const OutK& out, const 
   k_place_onehot<<<(unsigned)((n_rows + NT / 32 - 1) / (NT / 32)), NT, 0, s>>>(env, pc, pos, n_rows, out);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
-  if (out.noise != nullptr || out.spikes != nullptr) {
-    const int np128 = (pc.n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
-    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, pc.n_cells, np128, n_rows);
-    g_launches++;
-    RIAB_CUDA_OK(cudaGetLastError());
-  }
-  return 0;
+  return finish_rows(out, pc.n_cells, n_rows, s);
 }
 
+// PlaceCells other than one_hot (launch_onehot)
 template <int MODE>
 int launch_place(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
                  const PlaceConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s,
-                 const RunK* run = nullptr) {
-  if (pc.desc == RIAB_PC_ONE_HOT) {
-    if (MODE != 0) return fail(RIAB_ERR_INVALID, "one_hot is launched unfused");
-    return launch_onehot(env, pc, out, pos_in, n_rows, s);
-  }
+                 const RunK* run) {
   // the common Gaussian profile without geodesic detours gets a compile-time specialisation
   if (pc.desc == RIAB_PC_GAUSSIAN && pc.geometry != RIAB_GEOM_GEODESIC)
-    return launch_place_d<MODE, RIAB_PC_GAUSSIAN>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  return launch_place_d<MODE, -1>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    return launch_walls<PlacePolicy, MODE, RIAB_PC_GAUSSIAN>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  return launch_walls<PlacePolicy, MODE, -1>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
 }
 
 // PhasePrecessingPlaceCells: the run-time description profile only, MODE 0 / 1 / 2 (no whole run)
@@ -2009,19 +2010,7 @@ template <int MODE>
 int launch_pppc(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io,
                 const PppcConst& pc, const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s) {
   static_assert(MODE <= 2, "phase precessing place cells have no whole-run launch");
-  const int wi = pc.n_inner;
-  if (pc.comp) {
-    if (wi == 0) return launch_tile<PppcPolicy<0, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-    if (wi == 1) return launch_tile<PppcPolicy<1, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-    if (wi == 2) return launch_tile<PppcPolicy<2, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-    if (wi <= 4) return launch_tile<PppcPolicy<4, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-    return launch_tile<PppcPolicy<8, -1, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-  }
-  if (wi == 0) return launch_tile<PppcPolicy<0, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-  if (wi == 1) return launch_tile<PppcPolicy<1, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-  if (wi == 2) return launch_tile<PppcPolicy<2, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-  if (wi <= 4) return launch_tile<PppcPolicy<4, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
-  return launch_tile<PppcPolicy<8, -1>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s);
+  return launch_walls<PppcPolicy, MODE, -1>(env, ag, mp, io, pc, out, pos_in, n_rows, s, nullptr);
 }
 
 // riab_run pipelines BoundaryVectorCells across steps: the float64 ray kernel of step s+1 (latency-bound, FP64 pipe) runs
@@ -2090,9 +2079,8 @@ int launch_bvc(const EnvK& env, const riab_bvc_cells* bvc, const OutK& out, cons
   }
   // (the attribute belongs to the current device's function image: set per call, a single process may drive several GPUs)
   RIAB_CUDA_OK(cudaFuncSetAttribute(k_bvc_integrate, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  int dev = 0, sms = 0;
-  RIAB_CUDA_OK(cudaGetDevice(&dev));
-  RIAB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms, rc;
+  if ((rc = num_sms(sms))) return rc;
   const unsigned cts = (unsigned)(bc.n_pad / BVC_CT);
   unsigned gy = (unsigned)((2 * sms + cts - 1) / cts);           // ~2 CTAs per SM in total
   if (gy > n_tiles) gy = (unsigned)n_tiles;
@@ -2106,12 +2094,7 @@ int launch_bvc(const EnvK& env, const riab_bvc_cells* bvc, const OutK& out, cons
   }
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
-  if (out.noise != nullptr || (out.spikes != nullptr && !fold)) {
-    const int np128 = (bc.n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
-    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, bc.n_cells, np128, n_rows);
-    g_launches++;
-    RIAB_CUDA_OK(cudaGetLastError());
-  }
+  if (!fold && (rc = finish_rows(out, bc.n_cells, n_rows, s))) return rc;
   if (pipe) {
     RIAB_CUDA_OK(cudaEventRecord(pipe->int_done[pb][out.pop], s));
     pipe->used[pb][out.pop] = true;
@@ -2202,14 +2185,7 @@ int launch_ffl(const riab_ffl_cells* f, long long n_rows, const double* pos, con
   if (bn == 8) rc = launch_ffl_bn<8>(k, s);
   else if (bn == 32) rc = launch_ffl_bn<32>(k, s);
   else rc = launch_ffl_bn<64>(k, s);
-  if (rc) return rc;
-  if (out.noise != nullptr || out.spikes != nullptr) {
-    const int np128 = (f->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
-    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, f->n_cells, np128, n_rows);
-    g_launches++;
-    RIAB_CUDA_OK(cudaGetLastError());
-  }
-  return 0;
+  return rc ? rc : finish_rows(out, f->n_cells, n_rows, s);
 }
 
 // ---------------------------------------------------------------------------
@@ -2218,6 +2194,22 @@ long long nnn_w1_offset(const riab_nnn_cells* c, int i) {
   long long off = 0;
   for (int j = 0; j < i; ++j) off += 2LL * ((c->widths[1] + 7) / 8 * 8) * ((c->inputs[j].n_in + FFL_BK - 1) / FFL_BK * FFL_BK);
   return off;
+}
+
+// The layer widths and activations of a module with n_layers >= 1 and inputs of n_in > 0 rates each, as riab_nnn_pack
+// packs them and the kernels run them; who: the messages' prefix.
+int check_nnn_layers(const riab_nnn_cells* c, const char* who) {
+  int n_in = 0;
+  for (int i = 0; i < c->n_inputs; ++i) n_in += c->inputs[i].n_in;
+  if (n_in != c->widths[0]) return fail(RIAB_ERR_INVALID, "%s: inputs give %d rates, widths[0] is %d", who, n_in, c->widths[0]);
+  for (int l = 1; l <= c->n_layers; ++l) {
+    if (c->widths[l] <= 0) return fail(RIAB_ERR_INVALID, "%s: width %d of layer %d", who, c->widths[l], l);
+    if (l < c->n_layers && c->widths[l] > RIAB_NNN_MAX_HIDDEN)
+      return fail(RIAB_ERR_UNSUPPORTED, "%s: hidden width %d (at most %d)", who, c->widths[l], RIAB_NNN_MAX_HIDDEN);
+    if (c->act[l - 1] < RIAB_NNN_IDENTITY || c->act[l - 1] > RIAB_NNN_TANH)
+      return fail(RIAB_ERR_INVALID, "%s: bad activation %d", who, c->act[l - 1]);
+  }
+  return 0;
 }
 
 int check_nnn(const riab_nnn_cells* c, long long n_rows) {
@@ -2233,21 +2225,14 @@ int check_nnn(const riab_nnn_cells* c, long long n_rows) {
     return 0;
   }
   if (c->packed_dev == nullptr || ((uintptr_t)c->packed_dev) % 16 != 0) return fail(RIAB_ERR_INVALID, "nnn: packed_dev NULL or misaligned");
-  int n_in = 0;
   for (int i = 0; i < c->n_inputs; ++i) {
     const riab_ffl_input& in = c->inputs[i];
     if (in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || (in.rows_dev != nullptr && in.ld < in.n_in))
       return fail(RIAB_ERR_INVALID, "nnn input %d: bad sizes (pack with riab_nnn_pack)", i);
     if (((uintptr_t)in.rows_dev) % 16 != 0 || (in.ld * 4) % 16 != 0) return fail(RIAB_ERR_INVALID, "NNN inputs need 16-byte aligned rows");
-    n_in += in.n_in;
   }
-  if (n_in != c->widths[0]) return fail(RIAB_ERR_INVALID, "nnn: inputs give %d rates, widths[0] is %d", n_in, c->widths[0]);
-  for (int l = 1; l <= c->n_layers; ++l) {
-    if (c->widths[l] <= 0) return fail(RIAB_ERR_INVALID, "nnn: width %d of layer %d", c->widths[l], l);
-    if (l < c->n_layers && c->widths[l] > RIAB_NNN_MAX_HIDDEN)
-      return fail(RIAB_ERR_UNSUPPORTED, "nnn: hidden width %d (at most %d)", c->widths[l], RIAB_NNN_MAX_HIDDEN);
-    if (c->act[l - 1] < RIAB_NNN_IDENTITY || c->act[l - 1] > RIAB_NNN_TANH) return fail(RIAB_ERR_INVALID, "nnn: bad activation %d", c->act[l - 1]);
-  }
+  int rc;
+  if ((rc = check_nnn_layers(c, "nnn"))) return rc;
   if (c->widths[c->n_layers] != c->n_cells) return fail(RIAB_ERR_INVALID, "nnn: n_cells != the last layer's width");
   return 0;
 }
@@ -2287,13 +2272,7 @@ int launch_nnn(const riab_nnn_cells* c, long long n_rows, const double* pos, con
     RIAB_CUDA_OK(nnn_launch(k, bn, s));
     g_launches++;
   }
-  if (out.noise != nullptr || out.spikes != nullptr) {
-    const int np128 = (c->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
-    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, c->n_cells, np128, n_rows);
-    g_launches++;
-    RIAB_CUDA_OK(cudaGetLastError());
-  }
-  return 0;
+  return finish_rows(out, c->n_cells, n_rows, s);
 }
 
 // ---------------------------------------------------------------------------
@@ -2431,14 +2410,7 @@ int launch_rsn(const riab_rsn_cells* r, const PlaceConst& pc, const EnvK& env, c
   else if (wi == 2) rc = launch_rsn_bn<2, RIAB_PC_GAUSSIAN>(k, s);
   else if (wi <= 4) rc = launch_rsn_bn<4, RIAB_PC_GAUSSIAN>(k, s);
   else rc = launch_rsn_bn<8, RIAB_PC_GAUSSIAN>(k, s);
-  if (rc) return rc;
-  if (out.noise != nullptr || out.spikes != nullptr) {
-    const int np128 = (r->n_cells + CELL_PAD - 1) / CELL_PAD * CELL_PAD;
-    k_finish_rows<<<dim3((unsigned)n_rows, (unsigned)((np128 / 4 + NT - 1) / NT)), NT, 0, s>>>(out, r->n_cells, np128, n_rows);
-    g_launches++;
-    RIAB_CUDA_OK(cudaGetLastError());
-  }
-  return 0;
+  return rc ? rc : finish_rows(out, r->n_cells, n_rows, s);
 }
 
 int make_src(const riab_motion_source* src, long long n_agents, SrcK& k) {
@@ -2470,6 +2442,8 @@ const riab_step_io kNoStep = {};
 // One population of one step, checked: its kind's constants and its output.
 struct Pop {
   int kind = -1, n_cells = 0;
+  int n_pad = 0;                        // the k_step kinds' packed cell count (a multiple of CELL_PAD), else 0
+  bool step_policy = false;             // has_step_policy
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
   PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc; PppcConst pppc; PwnConst pwn;
@@ -2480,24 +2454,35 @@ struct Pop {
   const riab_nnn_cells* nnn = nullptr;
 };
 
+// Whether a population's rates come from a k_step policy, so that a motion step can be fused into its rate kernel.  The
+// others: one_hot PlaceCells (an arg-min across cells), BVC (the latency-bound ray kernel wants all its CTAs in ONE wave:
+// the 128-register motion code would halve its occupancy), FeedForwardLayers and NeuralNetworkNeurons (they read other
+// populations' rows, not the positions) and RandomSpatialNeurons (a GEMM kernel without motion warps).
+bool has_step_policy(int kind, const void* cells) {
+  if (kind == RIAB_CELLS_PLACE) return cells != nullptr && ((const riab_place_cells*)cells)->description != RIAB_PC_ONE_HOT;
+  return kind == RIAB_CELLS_GRID || kind == RIAB_CELLS_OVC || kind == RIAB_CELLS_KIN || kind == RIAB_CELLS_AVC ||
+         kind == RIAB_CELLS_PPPC || kind == RIAB_CELLS_PWN;
+}
+
 int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* out, const riab_neuron_noise* noise,
              double dt, const riab_agents& ag, Pop& d) {
   if (cells == nullptr) return fail(RIAB_ERR_INVALID, "cells NULL");
   int rc = 0;
   d.kind = kind;
+  d.step_policy = has_step_policy(kind, cells);
   if (kind == RIAB_CELLS_PLACE) {
     const riab_place_cells* pc = (const riab_place_cells*)cells;
     rc = make_place(pc, ek, d.place);
-    d.n_cells = pc->n_cells;
+    d.n_cells = pc->n_cells; d.n_pad = d.place.n_pad;
     if (pc->description != RIAB_PC_ONE_HOT) d.bound = fmaxf(pc->min_fr, pc->max_fr);   // one_hot: post-pass spikes, dense
   } else if (kind == RIAB_CELLS_GRID) {
     const riab_grid_cells* gc = (const riab_grid_cells*)cells;
     rc = make_grid(gc, ek, d.grid);
-    d.n_cells = gc->n_cells;
+    d.n_cells = gc->n_cells; d.n_pad = d.grid.n_pad;
     d.bound = fmaxf(gc->min_fr, gc->max_fr);
   } else if (kind == RIAB_CELLS_OVC) {
     rc = make_ovc((const riab_ovc_cells*)cells, ek, ag.head_direction, d.ovc);
-    d.n_cells = d.ovc.n_cells;
+    d.n_cells = d.ovc.n_cells; d.n_pad = d.ovc.n_pad;
   } else if (kind == RIAB_CELLS_BVC) {
     d.bvc = (const riab_bvc_cells*)cells;
     d.n_cells = d.bvc->n_cells;
@@ -2514,17 +2499,17 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
     d.n_cells = d.rsn->n_cells;
   } else if (kind == RIAB_CELLS_KIN) {
     rc = make_kin((const riab_kin_cells*)cells, ag, d.kin);
-    d.n_cells = d.kin.n_cells;
+    d.n_cells = d.kin.n_cells; d.n_pad = d.kin.n_pad;
   } else if (kind == RIAB_CELLS_AVC) {
     rc = make_avc((const riab_avc_cells*)cells, ek, ag.head_direction, ag.n_agents, d.avc);
-    d.n_cells = d.avc.n_cells;
+    d.n_cells = d.avc.n_cells; d.n_pad = d.avc.n_pad;
   } else if (kind == RIAB_CELLS_PPPC) {
     rc = make_pppc((const riab_pppc_cells*)cells, ek, ag.velocity, d.pppc);
-    d.n_cells = ((const riab_pppc_cells*)cells)->place.n_cells;
+    d.n_cells = ((const riab_pppc_cells*)cells)->place.n_cells; d.n_pad = d.pppc.n_pad;
   } else if (kind == RIAB_CELLS_PWN) {
     const riab_pwn_cells* pw = (const riab_pwn_cells*)cells;
     rc = make_pwn(pw, d.pwn);
-    d.n_cells = pw->n_cells;
+    d.n_cells = pw->n_cells; d.n_pad = d.pwn.n_pad;
     d.bound = fmaxf(pw->min_fr, pw->max_fr);
   } else if (kind == RIAB_CELLS_NNN) {
     d.nnn = (const riab_nnn_cells*)cells;
@@ -2543,41 +2528,43 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
 bool ffl_like(int kind) { return kind == RIAB_CELLS_FFL || kind == RIAB_CELLS_TD || kind == RIAB_CELLS_NNN; }
 
 // One population's kernels for one step.  MODE 0: rates at the agents' positions; 1: the motion step fused in; 2: skewed
-// (rates at the current positions while the motion of the next step runs, riab_run).  BVC, FFL and RSN populations run
-// MODE 0.
+// (rates at the current positions while the motion of the next step runs, riab_run); 3 / 4: riab_run's whole run (run),
+// for the kinds whole_run_applies admits.  Kinds without a k_step policy run MODE 0 only.
 template <int MODE>
 int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const Pop& d,
-               cudaStream_t s, BvcPipe* pipe = nullptr) {
-  const double* pos_in = (MODE == 1) ? nullptr : ag.pos;
-  if (d.kind == RIAB_CELLS_PLACE) return launch_place<MODE>(ek, ag, mp, io, d.place, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_GRID)
-    return d.grid.turns ? launch_tile<GridPolicy<1>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s)
-                        : launch_tile<GridPolicy<0>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_PPPC) return launch_pppc<MODE>(ek, ag, mp, io, d.pppc, d.out, pos_in, ag.n_agents, s);
-  if (d.kind == RIAB_CELLS_PWN) return launch_tile<PwnPolicy, MODE>(ek, ag, mp, io, d.pwn, d.out, pos_in, ag.n_agents, s);
-  if constexpr (MODE == 0) {
-    if (d.kind == RIAB_CELLS_BVC)
-      return launch_bvc(ek, d.bvc, d.out, ag.pos, ag.n_agents, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
-    if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, ag.n_agents, d.out, s);
-    if (d.kind == RIAB_CELLS_NNN) return launch_nnn(d.nnn, ag.n_agents, ag.pos, d.out, s);
-    const int rc = launch_ffl(d.ffl, ag.n_agents, ag.pos, d.out, s);
-    return (rc || d.kind != RIAB_CELLS_TD) ? rc : launch_td_trace(d.td, ag.n_agents, d.out.rates, s);
-  } else {
+               cudaStream_t s, BvcPipe* pipe = nullptr, const RunK* run = nullptr) {
+  const double* pos_in = (MODE == 0 || MODE == 2) ? ag.pos : nullptr;
+  const long long n = ag.n_agents;
+  if (!d.step_policy) {
+    if constexpr (MODE == 0) {
+      if (d.kind == RIAB_CELLS_PLACE) return launch_onehot(ek, d.place, d.out, ag.pos, n, s);
+      if (d.kind == RIAB_CELLS_BVC)
+        return launch_bvc(ek, d.bvc, d.out, ag.pos, n, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
+      if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, n, d.out, s);
+      if (d.kind == RIAB_CELLS_NNN) return launch_nnn(d.nnn, n, ag.pos, d.out, s);
+      const int rc = launch_ffl(d.ffl, n, ag.pos, d.out, s);
+      return (rc || d.kind != RIAB_CELLS_TD) ? rc : launch_td_trace(d.td, n, d.out.rates, s);
+    }
     return fail(RIAB_ERR_INVALID, "cells kind %d is launched unfused", d.kind);
   }
+  if (d.kind == RIAB_CELLS_PLACE) return launch_place<MODE>(ek, ag, mp, io, d.place, d.out, pos_in, n, s, run);
+  if (d.kind == RIAB_CELLS_GRID)
+    return d.grid.turns ? launch_tile<GridPolicy<1>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, n, s, run)
+                        : launch_tile<GridPolicy<0>, MODE>(ek, ag, mp, io, d.grid, d.out, pos_in, n, s, run);
+  if constexpr (MODE <= 2) {
+    if (d.kind == RIAB_CELLS_OVC) return launch_tile<OvcPolicy, MODE>(ek, ag, mp, io, d.ovc, d.out, pos_in, n, s);
+    if (d.kind == RIAB_CELLS_KIN) return launch_tile<KinPolicy, MODE>(ek, ag, mp, io, d.kin, d.out, pos_in, n, s);
+    if (d.kind == RIAB_CELLS_AVC) return launch_tile<AvcPolicy, MODE>(ek, ag, mp, io, d.avc, d.out, pos_in, n, s);
+    if (d.kind == RIAB_CELLS_PPPC) return launch_pppc<MODE>(ek, ag, mp, io, d.pppc, d.out, pos_in, n, s);
+  }
+  if (d.kind == RIAB_CELLS_PWN) return launch_tile<PwnPolicy, MODE>(ek, ag, mp, io, d.pwn, d.out, pos_in, n, s, run);
+  return fail(RIAB_ERR_INVALID, "cells kind %d has no whole-run launch", d.kind);
 }
 
-// The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), one_hot (an
-// arg-min across cells), BVC (the latency-bound ray kernel wants all its CTAs in ONE wave: the 128-register motion code
-// would halve its occupancy), FeedForwardLayers and NeuralNetworkNeurons (they read other populations' rows, not the
-// positions) and RandomSpatialNeurons (a GEMM kernel without motion warps).
+// The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), and those of
+// populations without a k_step policy.
 bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
-  return io.collision_mask || io.first_hit || io.n_iters || d.kind == RIAB_CELLS_BVC || d.kind == RIAB_CELLS_FFL ||
-         d.kind == RIAB_CELLS_TD || d.kind == RIAB_CELLS_RSN || d.kind == RIAB_CELLS_NNN ||
-         (d.kind == RIAB_CELLS_PLACE && d.place.desc == RIAB_PC_ONE_HOT);
+  return io.collision_mask || io.first_hit || io.n_iters || !d.step_policy;
 }
 
 // One motion step, then population d's rates at the new positions; everything is checked before.
@@ -2618,6 +2605,19 @@ int rates_at(int kind, const void* cells, const double* pos_dev, int64_t n_pos, 
   at.n_agents = n_pos; at.pos = (double*)pos_dev; at.head_direction = (double*)head_dir; at.velocity = (double*)velocity;
   if ((rc = make_pop(ek, kind, cells, &ro, nullptr, 1.0, at, d))) return rc;
   d.first_wall = first_wall;
+  return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
+}
+
+// riab_ffl_rates / riab_nnn_rates: a layer over n_rows rows of its inputs; pos_dev masks the rows whose x is NaN
+int layer_rates(int kind, const void* cells, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
+                const riab_rates_out* out, void* stream) {
+  EnvK ek;
+  memset(&ek, 0, sizeof(ek));                       // no walls: a layer reads its inputs' rows
+  riab_agents at = {};
+  at.n_agents = n_rows; at.pos = (double*)pos_dev; at.id_offset = noise ? noise->id_offset : 0;
+  Pop d;
+  int rc;
+  if ((rc = make_pop(ek, kind, cells, out, noise, noise ? noise->dt : 1.0, at, d))) return rc;
   return launch_pop<0>(ek, at, kNoMotion, kNoStep, d, (cudaStream_t)stream);
 }
 
@@ -2698,14 +2698,13 @@ int whole_run_applies(const EnvK& ek, const riab_agents& ag, const riab_motion_p
   if ((rc = make_pop(ek, pp.kind, pp.cells, &ro, &nz, prm.dt, ag, d))) return rc;
   const OutK& ok = d.out;
   const long long A = ag.n_agents;
-  const bool place = pp.kind == RIAB_CELLS_PLACE;
-  const int ct = (place ? d.place.n_pad : pp.kind == RIAB_CELLS_PWN ? d.pwn.n_pad : d.grid.n_pad) / 4;
+  const int ct = d.n_pad / 4;
   const bool rows_ok = ((A * ok.ld) % 4 == 0) && ((A * ok.spike_ld) % 4 == 0);        // every ring row stays 16-byte aligned
   const bool lean = ok.vec_ok && rows_ok && (d.n_cells % 4 == 0) && ct <= RW * 32 &&
                     (ok.spikes == nullptr || (ag.id_offset & 1) == 0) &&
                     (4 % lean_groups(ct, 8) == 0) && (4 % lean_groups(ct, 4) == 0);      // groups divide the 4 producers
   // with a spike ring of one row a producer's clear of step s+1's rows could land before the consumers' RED.OR of step s
-  yes = !(place && d.place.desc == RIAB_PC_ONE_HOT) && lean && (hist == nullptr || hist->ring == nullptr || hist->ring_rows > 0) &&
+  yes = d.step_policy && lean && (hist == nullptr || hist->ring == nullptr || hist->ring_rows > 0) &&
         (pp.spikes_ring == nullptr || pp.ring_rows >= 2);
   return 0;
 }
@@ -2732,14 +2731,11 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   // NaN, so an Agent with one keeps the plain schedule: the positions advance before any population of the step.
   bool any_ffl = false;
   for (int p = 0; p < n_pops; ++p) any_ffl = any_ffl || ffl_like(pops[p].kind);
-  const bool onehot0 = n_pops >= 1 && pops[0].kind == RIAB_CELLS_PLACE && pops[0].cells != nullptr &&
-                       ((const riab_place_cells*)pops[0].cells)->description == RIAB_PC_ONE_HOT;
-  // Skewed schedule (population 0 is a Place / Grid / OVC / kinematic / AVC population): motion(0) alone, then per step one kernel that
-  // evaluates rates(s) of the current positions while its producer warps already run motion(s+1); the last step is rates
-  // only.  Same results as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source
-  // keeps the plain schedule (its motion kernel is cheap next to the rates).
-  const bool skew = n_pops >= 1 && pops[0].kind != RIAB_CELLS_BVC && pops[0].kind != RIAB_CELLS_RSN && !onehot0 && !any_ffl &&
-                    io.xi == nullptr &&
+  // Skewed schedule (population 0 has a k_step policy): motion(0) alone, then per step one kernel that evaluates rates(s)
+  // of the current positions while its producer warps already run motion(s+1); the last step is rates only.  Same results
+  // as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source keeps the plain
+  // schedule (its motion kernel is cheap next to the rates).
+  const bool skew = n_pops >= 1 && has_step_policy(pops[0].kind, pops[0].cells) && !any_ffl && io.xi == nullptr &&
                     !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr;
   plan.sched = skew ? RunPlan::SKEWED : RunPlan::PLAIN;
   plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || ffl_like(pops[0].kind));
@@ -2771,7 +2767,6 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
   cudaStream_t s = (cudaStream_t)stream;
   if (plan.sched == RunPlan::WHOLE) {
     const riab_population& pp = pops[0];
-    const Pop& d = plan.whole;
     RunK run;
     memset(&run, 0, sizeof(run));
     run.n_steps = n_steps;
@@ -2783,17 +2778,8 @@ int run_impl(const riab_agents* agents, const riab_env* env, const riab_motion_p
     riab_step_io io0 = *io;
     io0.history_row = nullptr;
     if (src != nullptr && (rc = make_src(src, A, run.src))) return rc;
-    if (pp.kind == RIAB_CELLS_PLACE)
-      return src ? launch_place<4>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run)
-                 : launch_place<3>(ek, *agents, *prm, io0, d.place, d.out, nullptr, A, s, &run);
-    if (pp.kind == RIAB_CELLS_PWN)
-      return src ? launch_tile<PwnPolicy, 4>(ek, *agents, *prm, io0, d.pwn, d.out, nullptr, A, s, &run)
-                 : launch_tile<PwnPolicy, 3>(ek, *agents, *prm, io0, d.pwn, d.out, nullptr, A, s, &run);
-    if (d.grid.turns)
-      return src ? launch_tile<GridPolicy<1>, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
-                 : launch_tile<GridPolicy<1>, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
-    return src ? launch_tile<GridPolicy<0>, 4>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run)
-               : launch_tile<GridPolicy<0>, 3>(ek, *agents, *prm, io0, d.grid, d.out, nullptr, A, s, &run);
+    return src ? launch_pop<4>(ek, *agents, *prm, io0, plan.whole, s, nullptr, &run)
+               : launch_pop<3>(ek, *agents, *prm, io0, plan.whole, s, nullptr, &run);
   }
 
   riab_motion_source src_st;                          // step st's clock: t_st = t_{st-1} + dt
@@ -3085,9 +3071,8 @@ int riab_history_rate_maps(const riab_history_view* h, const double* edges_x_dev
   if (h->rates_ring != nullptr) RIAB_CUDA_OK(cudaMemsetAsync(sum_dev, 0, bins * (size_t)h->ld * sizeof(double), s));
   const long long n_samples = h->n_steps * h->n_agents;
   if (n_samples == 0) return 0;
-  int dev = 0, sms = 0;
-  RIAB_CUDA_OK(cudaGetDevice(&dev));
-  RIAB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms, rc;
+  if ((rc = num_sms(sms))) return rc;
   long long blocks = (n_samples + NT / 32 - 1) / (NT / 32);
   if (blocks > sms * 8ll) blocks = sms * 8ll;
   k_history_maps<<<(unsigned)blocks, NT, 0, s>>>(*h, edges_x_dev, n_edges_x, edges_y_dev, n_edges_y, sum_dev,
@@ -3748,11 +3733,7 @@ int riab_ffl_pack(const double* w, int32_t n, int32_t n_in, riab_ffl_input* meta
 int riab_ffl_rates(const riab_ffl_cells* ffl, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
                    const riab_rates_out* out, void* stream) {
   if (ffl == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_ffl_rates: bad argument");
-  OutK ok;
-  int rc;
-  if ((rc = make_out(out, noise, ffl->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
-      (rc = check_ffl(ffl, ok, n_rows))) return rc;
-  return launch_ffl(ffl, n_rows, pos_dev, ok, (cudaStream_t)stream);
+  return layer_rates(RIAB_CELLS_FFL, ffl, n_rows, pos_dev, noise, out, stream);
 }
 
 // ------------------------------------------------------------ NeuralNetworkNeurons
@@ -3774,19 +3755,11 @@ int riab_nnn_pack(const double* params, riab_nnn_cells* meta, float* out) {
     return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: %d Linear layers (1 to %d)", L, RIAB_NNN_MAX_LAYERS);
   if (meta->n_inputs < 1 || meta->n_inputs > RIAB_FFL_MAX_INPUTS)
     return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: %d inputs (1 to %d)", meta->n_inputs, RIAB_FFL_MAX_INPUTS);
-  int n_in = 0;
-  for (int i = 0; i < meta->n_inputs; ++i) {
+  for (int i = 0; i < meta->n_inputs; ++i)
     if (meta->inputs[i].n_in <= 0) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: input %d has %d rates", i, meta->inputs[i].n_in);
-    n_in += meta->inputs[i].n_in;
-  }
-  if (n_in != meta->widths[0]) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: inputs give %d rates, widths[0] is %d", n_in, meta->widths[0]);
-  for (int l = 1; l <= L; ++l) {
-    if (meta->widths[l] <= 0) return fail(RIAB_ERR_INVALID, "riab_nnn_pack: width %d of layer %d", meta->widths[l], l);
-    if (l < L && meta->widths[l] > RIAB_NNN_MAX_HIDDEN)
-      return fail(RIAB_ERR_UNSUPPORTED, "riab_nnn_pack: hidden width %d (at most %d)", meta->widths[l], RIAB_NNN_MAX_HIDDEN);
-    if (meta->act[l - 1] < RIAB_NNN_IDENTITY || meta->act[l - 1] > RIAB_NNN_TANH)
-      return fail(RIAB_ERR_INVALID, "riab_nnn_pack: bad activation %d", meta->act[l - 1]);
-  }
+  int rc;
+  if ((rc = check_nnn_layers(meta, "riab_nnn_pack"))) return rc;
+  const int n_in = meta->widths[0];
   // layer 1: W_1's column block of each input through riab_ffl_pack
   const int h1 = meta->widths[1];
   const double* p = params;
@@ -3799,7 +3772,6 @@ int riab_nnn_pack(const double* params, riab_nnn_cells* meta, float* out) {
     for (int r = 0; r < h1; ++r)
       for (int j = 0; j < ni; ++j) block[(size_t)r * ni + j] = p[(size_t)r * n_in + col0 + j];
     riab_ffl_input tmp = meta->inputs[i];
-    int rc;
     if ((rc = riab_ffl_pack(block.data(), h1, ni, &tmp, o))) return rc;
     meta->inputs[i].k_pad = tmp.k_pad;
     o += riab_ffl_pack_floats(h1, ni);
@@ -3827,11 +3799,7 @@ int riab_nnn_pack(const double* params, riab_nnn_cells* meta, float* out) {
 int riab_nnn_rates(const riab_nnn_cells* cells, int64_t n_rows, const double* pos_dev, const riab_neuron_noise* noise,
                    const riab_rates_out* out, void* stream) {
   if (cells == nullptr || n_rows < 0) return fail(RIAB_ERR_INVALID, "riab_nnn_rates: bad argument");
-  OutK ok;
-  int rc;
-  if ((rc = make_out(out, noise, cells->n_cells, noise ? noise->dt : 1.0, noise ? noise->id_offset : 0, ok)) ||
-      (rc = check_nnn(cells, n_rows))) return rc;
-  return launch_nnn(cells, n_rows, pos_dev, ok, (cudaStream_t)stream);
+  return layer_rates(RIAB_CELLS_NNN, cells, n_rows, pos_dev, noise, out, stream);
 }
 
 // ------------------------------------------------------------------ TD learning
