@@ -572,7 +572,17 @@ int riab_avc_rates(const double* pos_dev, int64_t n_pos, const double* other_pos
  *   W_l += dt eta (sum_a outer(td_a * phi'_a, e_{a,l}) / n_rows) - eta dt L2 W_l
  * to float64 master weights, then rewrites the layer's W_hi | W_lo blocks (riab_ffl_pack of the new master, bit for
  * bit).  The contraction runs over the row (agent) axis in fixed-size chunks whose float64 partial tiles are summed in
- * a fixed order: no atomics, the same inputs give the same weights. */
+ * a fixed order: no atomics, the same inputs give the same weights.
+ *
+ * Per-agent weights (per_agent_weights = 1): every row a is an independent learner with its own masters
+ * w_master_dev[l] (A, n_cells, n_in) f64, and the layer's contraction reads them directly (k_td_forward_pa):
+ *   V[a, j] = sum_l W_l[a, j, :] . I_l[a, :] + b_j   (float64 accumulation, then the layer's activation and phi')
+ * update_weights applies each row's own reference update, nothing averaged:
+ *   td   = reward + deriv - fr_prev / tau
+ *   W_l[a] += (dt eta) outer(td_a phi'_a, e_{a,l}) - (eta dt L2) W_l[a]
+ * elementwise in the reference's operation order (contribs/ValueNeuron.py:94-100), in non-contracting float64 from the
+ * float32 td, phi' and traces.  There is no W_hi | W_lo block (ffl.inputs[l].w_dev is not read and may be NULL), no
+ * scratch and no split of the agent axis. */
 typedef struct {
   riab_ffl_cells ffl;                       /* the layer; ffl.inputs[l].w_dev is the W_hi | W_lo block the learning rewrites */
   float* fr_prev_dev;                       /* (A, ld) f32: firingrate of the last update (zeros before it and after reset) */
@@ -581,25 +591,37 @@ typedef struct {
   int64_t ld;                               /* row stride of the layer's rates, fr_prev, deriv and td_error (floats) */
   float* trace_dev[RIAB_FFL_MAX_INPUTS];    /* (A, trace_ld[l]) f32 eligibility trace of ffl.inputs[l] */
   int64_t trace_ld[RIAB_FFL_MAX_INPUTS];    /* multiple of 4, >= ffl.inputs[l].n_in */
-  double* w_master_dev[RIAB_FFL_MAX_INPUTS];/* (n_cells, n_in) f64 row-major master weights of ffl.inputs[l] */
+  double* w_master_dev[RIAB_FFL_MAX_INPUTS];/* (n_cells, n_in) f64 row-major master weights of ffl.inputs[l];
+                                               per_agent_weights: (A, n_cells, n_in), agent a's block at a n_cells n_in */
   double dt, tau, tau_e, eta, L2;           /* Agent.dt and the ValueNeuron params; tau_e > 0 */
   int32_t self_input;                       /* index of the input that is the layer itself (it reads fr_prev), or -1 */
-  int32_t reserved;
+  union {
+    int32_t per_agent_weights;              /* 0: one weight matrix per input shared by the rows; 1: one per row (agent) */
+    int32_t reserved;                       /* the field's former name */
+  };
 } riab_td_cells;
 typedef enum { RIAB_TD_REWARD_SHARED = 0 /* (n_cells) f64, every row */, RIAB_TD_REWARD_ROWS = 1 /* (n_rows, ld) f32 */
 } riab_td_reward_mode;
 /* Number of agent chunks riab_td_learn splits the contraction of one input (n_in) into: float64 partial tiles of
- * n_cells x n_in each, summed in a fixed order.  Depends on the shapes only. */
+ * n_cells x n_in each, summed in a fixed order.  Depends on the shapes only.  Shared weights only: the per-agent
+ * update has no contraction over the agents. */
 int64_t riab_td_splits(int32_t n_cells, int32_t n_in, int64_t n_rows);
-/* Device scratch riab_td_learn needs for n_rows rows (bytes). */
+/* Device scratch riab_td_learn needs for n_rows rows (bytes); 0 with per_agent_weights. */
 int64_t riab_td_scratch_bytes(const riab_td_cells* cells, int64_t n_rows);
 /* ValueNeuron.update_weights(reward) over n_rows rows: td -> td_error_out (n_rows, ld) f32, then every input's master
- * and W_hi | W_lo.  scratch: riab_td_scratch_bytes device bytes, 16-byte aligned. */
+ * and W_hi | W_lo (shared weights), or each row's own masters (per_agent_weights, n_rows = the masters' A).  scratch:
+ * riab_td_scratch_bytes device bytes, 16-byte aligned (may be NULL with per_agent_weights). */
 int riab_td_learn(const riab_td_cells* cells, int64_t n_rows, const void* reward, int32_t reward_mode, float* td_error_out,
                   void* scratch, void* stream);
 /* ValueNeuron.reset (:106-113): zero fr_prev, deriv, td_error and the traces of the rows whose mask byte is non-zero
  * (mask (A) uint8 device, NULL = every row). */
 int riab_td_reset(const riab_td_cells* cells, int64_t n_rows, const uint8_t* mask, void* stream);
+/* The per-agent layer's rates away from the agents' step (get_state at positions, for chosen agents): row r is
+ *   out[r] = phi(sum_l W_l[weight_agent_of_row[r]] . I_l[input_row_of_row[r]] + b)
+ * with I_l = cells->ffl.inputs[l].rows_dev (rows of ld ffl.inputs[l].ld; NULL = zeros).  A NULL map is the identity.
+ * out_dev (n_rows, ld_out) f32; firingrate_prime, noise and spikes are not touched.  Needs per_agent_weights. */
+int riab_td_rates_pa(const riab_td_cells* cells, int64_t n_rows, const int64_t* weight_agent_of_row_dev,
+                     const int64_t* input_row_of_row_dev, float* out_dev, int64_t ld_out, void* stream);
 
 /* ------------------------------------ PhasePrecessingPlaceCells (RIAB_CELLS_PPPC)
  * contribs/PhasePrecessingPlaceCells.py:66-119: at the agents, the PlaceCells rate of `place` times the theta modulation

@@ -1145,30 +1145,37 @@ class FeedForwardLayer(Neurons):
         else:
             fc = _lib.FflCells.from_buffer_copy(c)
             fc.prime_dev = None
-            keep = []
-            n_pos = self._n_pos(evaluate_at, kwargs, self.Agent.n_agents)
-            for i, e in enumerate(self.inputs.values()):
-                pass_max = max_recurrence
-                if max_recurrence is not None and e["recurrent"]:
-                    if max_recurrence <= 0:
-                        fc.inputs[i].rows_dev = None                  # skipped: contributes nothing (Neurons.py:2812-2815)
-                        continue
-                    pass_max = max_recurrence - 1
-                I = e["layer"].get_state(evaluate_at, max_recurrence=pass_max, return_tensor=True, **kwargs)
-                if I.dtype != torch.float32 or I.stride(1) != 1 or I.stride(0) % 4 or I.data_ptr() % 16:
-                    ld = (I.shape[1] + 3) // 4 * 4
-                    J = torch.zeros((I.shape[0], ld), dtype=torch.float32, device=self.device)
-                    J[:, : I.shape[1]] = I
-                    I = J
-                assert I.shape[0] == n_pos
-                keep.append(I)
-                fc.inputs[i].rows_dev, fc.inputs[i].ld = I.data_ptr(), I.stride(0)
+            n_pos, keep = self._input_rows(fc, evaluate_at, max_recurrence, kwargs)
         out = torch.empty((n_pos, self._ld()), dtype=torch.float32, device=self.device)
         ro = _lib.RatesOut()
         ro.rates_row, ro.ld = out.data_ptr(), self._ld()
         _lib.check(self._lib.riab_ffl_rates(C.byref(fc), n_pos, None, None, C.byref(ro), self.Agent._stream()))
         r = self._result(out, return_tensor)
         return r[:, 0] if (evaluate_at == "last" and n_pos == 1 and not return_tensor) else r
+
+    def _input_rows(self, fc, evaluate_at, max_recurrence, kwargs):
+        """Point fc's inputs at their populations' get_state(evaluate_at, ...) rows, evaluated on the device.  Returns the
+        row count and the tensors that must outlive the evaluation."""
+        torch = self._torch
+        keep = []
+        n_pos = self._n_pos(evaluate_at, kwargs, self.Agent.n_agents)
+        for i, e in enumerate(self.inputs.values()):
+            pass_max = max_recurrence
+            if max_recurrence is not None and e["recurrent"]:
+                if max_recurrence <= 0:
+                    fc.inputs[i].rows_dev = None                  # skipped: contributes nothing (Neurons.py:2812-2815)
+                    continue
+                pass_max = max_recurrence - 1
+            I = e["layer"].get_state(evaluate_at, max_recurrence=pass_max, return_tensor=True, **kwargs)
+            if I.dtype != torch.float32 or I.stride(1) != 1 or I.stride(0) % 4 or I.data_ptr() % 16:
+                ld = (I.shape[1] + 3) // 4 * 4
+                J = torch.zeros((I.shape[0], ld), dtype=torch.float32, device=self.device)
+                J[:, : I.shape[1]] = I
+                I = J
+            assert I.shape[0] == n_pos
+            keep.append(I)
+            fc.inputs[i].rows_dev, fc.inputs[i].ld = I.data_ptr(), I.stride(0)
+        return n_pos, keep
 
 
 # =============================================================================

@@ -133,10 +133,13 @@ class TdCells(C.Structure):
                 ("ld", C.c_int64), ("trace_dev", C.c_void_p * FFL_MAX_INPUTS), ("trace_ld", C.c_int64 * FFL_MAX_INPUTS),
                 ("w_master_dev", C.c_void_p * FFL_MAX_INPUTS), ("dt", C.c_double), ("tau", C.c_double),
                 ("tau_e", C.c_double), ("eta", C.c_double), ("L2", C.c_double), ("self_input", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("per_agent_weights", C.c_int32)]
     # FeedForwardLayer's host code reaches the embedded layer's fields through these (they share the struct's memory)
     inputs = property(lambda self: self.ffl.inputs)
     prime_dev = property(lambda self: self.ffl.prime_dev, lambda self, v: setattr(self.ffl, "prime_dev", v))
+
+
+TdCells.reserved = TdCells.per_agent_weights      # the header's union keeps the field's former name
 
 
 TD_REWARD_SHARED, TD_REWARD_ROWS = 0, 1                       # riab_td_reward_mode
@@ -257,6 +260,8 @@ SYMBOLS = {
     "riab_td_scratch_bytes": (C.c_int64, [C.POINTER(TdCells), C.c_int64]),
     "riab_td_learn": (C.c_int, [C.POINTER(TdCells), C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "riab_td_reset": (C.c_int, [C.POINTER(TdCells), C.c_int64, C.c_void_p, C.c_void_p]),
+    "riab_td_rates_pa": (C.c_int, [C.POINTER(TdCells), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                   C.c_void_p]),
     "riab_rsn_pack_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "riab_rsn_pack": (C.c_int, [c_double_p, C.c_int32, c_double_p, C.c_int32, C.c_double, c_double_p, C.c_int32, C.c_int32,
                                 c_double_p, C.c_int32, C.POINTER(RsnCells), c_float_p, c_double_p]),

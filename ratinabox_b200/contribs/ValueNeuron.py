@@ -1,5 +1,6 @@
 """ratinabox.contribs.ValueNeuron (contribs/ValueNeuron.py:10-113) on the device: TD learning of a value function on a
-FeedForwardLayer, with per-agent eligibility traces and one weight matrix shared by the batch."""
+FeedForwardLayer, with per-agent eligibility traces and one weight matrix shared by the batch, or with
+``per_agent_weights`` one independent learner per agent."""
 import ctypes as C
 
 import numpy as np
@@ -34,7 +35,16 @@ class _TdInput(_FflInput):
         dict.__setitem__(self, k, v)
 
 
-class ValueNeuron(FeedForwardLayer):
+class _BatchLearning:
+    """The batch engine's ValueNeuron param, collected with the defaults like every class's ``default_params`` but kept
+    apart from ``ValueNeuron.default_params``, which stay the reference's.
+
+    ``per_agent_weights``: False (default) -- one weight matrix per input shared by the batch, learned from the mean of
+    the agents' updates; True -- every agent is an independent learner with its own weights (see ValueNeuron)."""
+    default_params = {"per_agent_weights": False}
+
+
+class ValueNeuron(FeedForwardLayer, _BatchLearning):
     """ratinabox.contribs.ValueNeuron: ``n`` value functions V = phi(sum_l w_l . I_l + b) learned by continuous TD,
 
         update():          firingrate_deriv = (firingrate - firingrate_last) / dt,  e_l <- dt I_l + (1 - dt / tau_e) e_l
@@ -54,7 +64,20 @@ class ValueNeuron(FeedForwardLayer):
 
     The weights are kept in float64 on the device (the L2 decay moves a weight by ~5e-8 of itself per step at the
     demo's values, under float32's half ulp) and re-split into the layer's error-compensated TF32 operands after each
-    learning step.  ``Agent.run`` runs ``update()`` (rates, derivative, traces) but never ``update_weights``."""
+    learning step.  ``Agent.run`` runs ``update()`` (rates, derivative, traces) but never ``update_weights``.
+
+    With ``params["per_agent_weights"] = True`` agent ``a`` of the batch IS the reference's single-agent ValueNeuron
+    driven by its own inputs and reward:
+
+    * every input's weights are ``(n_agents, n, n_in)`` float64 on the device (``8 n_agents sum n n_in`` bytes, checked
+      against the free device memory before anything is allocated: ``MemoryError``).  Construction draws the reference's
+      ``(n, n_in)`` weights and gives every agent a copy; ``inputs[name]["w"]`` reads ``(n_agents, n, n_in)`` (``(n,
+      n_in)`` for one agent) and takes ``(n, n_in)`` (every agent) or ``(n_agents, n, n_in)``;
+    * the rates contract each agent's own weights with its inputs in float64 (csrc/riab_td.cuh, k_td_forward_pa);
+    * ``update_weights`` applies each agent's own reference update, nothing averaged, with the same reward forms;
+    * ``get_state(evaluate_at="all" | None, pos=...)`` gives ``(n_agents, n, n_pos)`` (``(n, n_pos)`` for one agent), and
+      ``agents=[...]`` picks the learners evaluated: ``(len(agents), n, n_pos)``.  At "last" / "agent" each agent's
+      row uses its own weights, ``(n, n_agents)`` as for shared weights, and firingrate_prime is not refreshed."""
     default_params = {                                              # contribs/ValueNeuron.py:36-43
         "tau": 2,
         "tau_e": None,
@@ -73,6 +96,10 @@ class ValueNeuron(FeedForwardLayer):
         self._fr_prev = self._deriv = self._td = None
         self._scratch = None
         self._reward_keep = None
+        self._pa = bool(dict(params).get("per_agent_weights", False))
+        if self._pa:
+            n = int(dict(params).get("n", ValueNeuron.default_params["n"]))
+            self._check_memory(Agent, 8 * Agent.n_agents * n * sum(l.n for l in dict(params).get("input_layers", [])))
         super().__init__(Agent, params)
         if self.tau_e is None:                                      # :50-51
             self.tau_e = self.tau / 4
@@ -80,11 +107,25 @@ class ValueNeuron(FeedForwardLayer):
             dict.__setitem__(e, "eligibility_trace", None)          # :52-53: the inputs present now get a trace
 
     def add_input(self, input_layer, w=None, w_init_scale=1, recurrent=False, **kwargs):
+        if self._pa and input_layer.name not in getattr(self, "inputs", {}):
+            others = sum(e["layer"].n for e in getattr(self, "inputs", {}).values())
+            self._check_memory(self.Agent, 8 * self.Agent.n_agents * self.n * (others + input_layer.n))
         super().add_input(input_layer, w=w, w_init_scale=w_init_scale, recurrent=recurrent, **kwargs)
         name = input_layer.name
         for d in (self._master, self._w_pack, self._w_shadow, self._trace):
             d.pop(name, None)
         self.inputs[name] = _TdInput(self, name, self.inputs[name])
+
+    @staticmethod
+    def _check_memory(Agent, need):
+        """Refuse per-agent weights that would not fit in the device's free memory, before allocating them."""
+        import torch
+        if need <= 0 or Agent.device.type != "cuda":
+            return
+        free, _ = torch.cuda.mem_get_info(Agent.device)
+        if need > free:
+            raise MemoryError(f"per-agent weights need {need} bytes ({need / 1e9:.1f} GB) of device memory for "
+                              f"{Agent.n_agents} agents; {free} bytes are free")
 
     # ------------------------------------------------------------------ weights
     def _signature(self):
@@ -107,6 +148,12 @@ class ValueNeuron(FeedForwardLayer):
         f.bias_dev = self._bias_dev.data_ptr()
         for i, (name, e) in enumerate(self.inputs.items()):
             n_in = e["layer"].n
+            if self._pa:
+                if name not in self._master:
+                    self._master[name] = self._upload(self._w_full(name, dict.__getitem__(e, "w")))
+                f.inputs[i].n_in, f.inputs[i].k_pad = n_in, (n_in + 31) // 32 * 32
+                f.inputs[i].w_dev = None                            # the per-agent contraction reads the masters
+                continue
             if name not in self._master:
                 w = np.ascontiguousarray(dict.__getitem__(e, "w"), dtype=np.float64)
                 assert w.shape == (self.n, n_in), f"inputs[{name!r}]['w'] must have shape ({self.n}, {n_in})"
@@ -118,6 +165,16 @@ class ValueNeuron(FeedForwardLayer):
         f.n_inputs = len(self.inputs)
         return c
 
+    def _w_full(self, name, w):
+        """Per-agent weights: ``w`` ((n, n_in), every agent, or (n_agents, n, n_in)) as a C-contiguous (n_agents, n,
+        n_in) float64 array."""
+        A, n_in = self.Agent.n_agents, self.inputs[name]["n"]
+        w = np.asarray(w, dtype=np.float64)
+        if w.shape not in ((self.n, n_in), (A, self.n, n_in)):
+            raise ValueError(f"inputs[{name!r}]['w'] must have shape ({self.n}, {n_in}) or ({A}, {self.n}, {n_in}), "
+                             f"not {w.shape}")
+        return np.array(np.broadcast_to(w, (A, self.n, n_in)), order="C")            # an own, writable copy
+
     def _split(self, w, meta):
         host = np.zeros(self._lib.riab_ffl_pack_floats(self.n, w.shape[1]), dtype=np.float32)
         _lib.check(self._lib.riab_ffl_pack(_f64p(np.ascontiguousarray(w, dtype=np.float64)), self.n, w.shape[1],
@@ -125,11 +182,15 @@ class ValueNeuron(FeedForwardLayer):
         return host
 
     def _w_read(self, name, initial):
+        if name not in self._master and self._pa:
+            self._cells()                                   # per-agent weights: (A, n, n_in) from the first read on
         if name not in self._master:
             return initial                                  # not on the device yet: the array add_input stored
         sh = self._w_shadow.get(name)
         if sh is None:
             host = self._master[name].cpu().numpy()
+            if self._pa and self.Agent.n_agents == 1:
+                host = host[0]                                      # the squeeze rule: (n, n_in) for one agent
             sh = self._w_shadow[name] = [host, host.copy()]
         return sh[0]
 
@@ -143,11 +204,17 @@ class ValueNeuron(FeedForwardLayer):
 
     def _sync_weights(self):
         """Upload the weights the user edited in place or assigned since they were read (Agent._sync_user_writes)."""
-        for name, sh in self._w_shadow.items():
+        for name, sh in list(self._w_shadow.items()):
             if name not in self._master:
                 continue
             host, snap = sh
             if snap is not None and np.array_equal(host, snap, equal_nan=True):
+                continue
+            if self._pa:
+                self._master[name].copy_(self._torch.as_tensor(self._w_full(name, host)))
+                sh[1] = np.array(host, dtype=np.float64, copy=True)
+                if np.shape(host) != self._master[name].shape[self.Agent.n_agents == 1:]:
+                    del self._w_shadow[name]                        # broadcast: the next read copies the masters
                 continue
             w = np.ascontiguousarray(host, dtype=np.float64)
             assert w.shape == tuple(self._master[name].shape), \
@@ -183,6 +250,7 @@ class ValueNeuron(FeedForwardLayer):
             if e["layer"] is self:
                 c.self_input = i
         self._bind_self(c)
+        c.per_agent_weights = int(self._pa)
         c.dt, c.tau, c.tau_e = float(self.Agent.dt), float(self.tau), float(self.tau_e)
         c.eta, c.L2 = float(self.eta), float(self.L2)
         return c
@@ -237,6 +305,53 @@ class ValueNeuron(FeedForwardLayer):
                                                   device=self.device)
         v = np.broadcast_to(np.asarray(v, dtype=np.float64), (self.Agent.n_agents, n_in))
         self._trace[name][:, :n_in].copy_(self._torch.as_tensor(np.ascontiguousarray(v, dtype=np.float32)))
+
+    # --------------------------------------------------------------- get_state
+    def get_state(self, evaluate_at="last", max_recurrence=None, **kwargs):
+        """FeedForwardLayer.get_state; with per-agent weights see the class docstring (``agents=`` picks the learners
+        evaluated at "all" / ``pos``)."""
+        if not self._pa:
+            return super().get_state(evaluate_at, max_recurrence=max_recurrence, **kwargs)
+        torch, A, n = self._torch, self.Agent.n_agents, self.n
+        return_tensor = kwargs.pop("return_tensor", False)
+        agents = kwargs.pop("agents", None)
+        c = self._cells()
+        tc = _lib.TdCells.from_buffer_copy(c)
+        tc.ffl.prime_dev = None
+        per_row = evaluate_at in ("last", "agent")            # the points are the agents: row a uses agent a's weights
+        if per_row and agents is not None:
+            raise ValueError(f"agents= selects learners for get_state at positions, not at {evaluate_at!r}")
+        if evaluate_at == "last":
+            self.Agent._flush_pending()
+            n_pos = A
+        else:
+            if max_recurrence != 0 and any(e["layer"] is self for e in self.inputs.values()):
+                raise NotImplementedError("get_state away from the agents' rows of a per-agent ValueNeuron that is its "
+                                          "own input: pass max_recurrence=0")
+            n_pos, keep = self._input_rows(tc.ffl, evaluate_at, max_recurrence, kwargs)
+        sel = None
+        if per_row:
+            n_rows, w_row, in_row = n_pos, None, None
+        else:
+            sel = np.arange(A) if agents is None else np.asarray(agents, dtype=np.int64).reshape(-1)
+            if sel.size and (sel.min() < -A or sel.max() >= A):
+                raise IndexError(f"agent index out of range for {A} agents")
+            sel = np.where(sel < 0, sel + A, sel)
+            n_rows = sel.size * n_pos
+            w_row = torch.as_tensor(sel, device=self.device).repeat_interleave(n_pos)
+            in_row = torch.arange(n_pos, device=self.device, dtype=torch.int64).repeat(sel.size)
+        out = torch.empty((n_rows, self._ld()), dtype=torch.float32, device=self.device)
+        _lib.check(self._lib.riab_td_rates_pa(C.byref(tc), n_rows, None if w_row is None else w_row.data_ptr(),
+                                              None if in_row is None else in_row.data_ptr(), out.data_ptr(),
+                                              self._ld(), self.Agent._stream()))
+        if per_row:
+            r = self._result(out, return_tensor)
+            return r[:, 0] if (evaluate_at == "last" and n_pos == 1 and not return_tensor) else r
+        rows = out[:, :n].reshape(sel.size, n_pos, n)                      # (agents, n_pos, n)
+        if agents is None and A == 1:
+            rows = rows[0]
+            return rows if return_tensor else rows.T.contiguous().cpu().numpy().astype(np.float64)
+        return rows if return_tensor else rows.transpose(1, 2).contiguous().cpu().numpy().astype(np.float64)
 
     # ------------------------------------------------------------------ update
     def _check_update(self):

@@ -2140,7 +2140,8 @@ int launch_ffl_bn(FflK& k, cudaStream_t s) {
   return 0;
 }
 
-int check_ffl(const riab_ffl_cells* f, const OutK& out, long long n_rows) {
+// packed: the layer's contraction reads W_hi | W_lo blocks (every FeedForwardLayer but a per-agent TD layer)
+int check_ffl(const riab_ffl_cells* f, const OutK& out, long long n_rows, bool packed = true) {
   if (f == nullptr || f->bias_dev == nullptr) return fail(RIAB_ERR_INVALID, "ffl / bias_dev NULL");
   if (f->n_cells <= 0) return fail(RIAB_ERR_INVALID, "ffl: n_cells must be > 0");
   if (f->n_inputs < 0 || f->n_inputs > RIAB_FFL_MAX_INPUTS)
@@ -2151,7 +2152,7 @@ int check_ffl(const riab_ffl_cells* f, const OutK& out, long long n_rows) {
   for (int i = 0; i < f->n_inputs; ++i) {
     const riab_ffl_input& in = f->inputs[i];
     if (in.rows_dev == nullptr) continue;                        // an input that was never updated contributes zeros
-    if (in.w_dev == nullptr || in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || in.ld < in.n_in)
+    if ((packed && in.w_dev == nullptr) || in.n_in <= 0 || in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK || in.ld < in.n_in)
       return fail(RIAB_ERR_INVALID, "ffl input %d: bad weights / sizes (pack with riab_ffl_pack)", i);
     if (((uintptr_t)in.rows_dev) % 16 != 0 || (in.ld * 4) % 16 != 0 || ((uintptr_t)in.w_dev) % 16 != 0)
       return fail(RIAB_ERR_INVALID, "FFL operands need 16-byte aligned rows");
@@ -2287,10 +2288,13 @@ int check_td(const riab_td_cells* t, long long out_ld) {
   if (!(t->dt > 0.0) || !(t->tau_e > 0.0) || !std::isfinite(t->tau_e) || !std::isfinite(t->dt))
     return fail(RIAB_ERR_INVALID, "td: dt and tau_e must be finite and > 0");
   if (t->self_input < -1 || t->self_input >= f.n_inputs) return fail(RIAB_ERR_INVALID, "td: bad self_input %d", t->self_input);
+  if (t->per_agent_weights != 0 && t->per_agent_weights != 1)
+    return fail(RIAB_ERR_INVALID, "td: per_agent_weights must be 0 or 1, not %d", t->per_agent_weights);
   if (f.n_inputs < 0 || f.n_inputs > RIAB_FFL_MAX_INPUTS) return fail(RIAB_ERR_UNSUPPORTED, "td: %d inputs", f.n_inputs);
   for (int l = 0; l < f.n_inputs; ++l) {
     const riab_ffl_input& in = f.inputs[l];
-    if (t->trace_dev[l] == nullptr || t->w_master_dev[l] == nullptr || in.w_dev == nullptr || in.n_in <= 0 ||
+    if (t->trace_dev[l] == nullptr || t->w_master_dev[l] == nullptr || (!t->per_agent_weights && in.w_dev == nullptr) ||
+        in.n_in <= 0 ||
         in.k_pad != (in.n_in + FFL_BK - 1) / FFL_BK * FFL_BK)
       return fail(RIAB_ERR_INVALID, "td input %d: trace / master / packed weights missing or mis-sized", l);
     if (t->trace_ld[l] < in.n_in || t->trace_ld[l] % 4 != 0 || ((uintptr_t)t->trace_dev[l]) % 16 != 0)
@@ -2316,6 +2320,42 @@ int launch_td_trace(const riab_td_cells* t, long long n_rows, const float* rates
   k.dt = (float)t->dt;
   k.decay = (float)(1.0 - t->dt / t->tau_e);
   k_td_trace<<<(unsigned)n_rows, TD_TRACE_THREADS, 0, s>>>(k);
+  g_launches++;
+  RIAB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// The per-agent layer's contraction over n_rows rows (k_td_forward_pa): row r reads the masters of agent w_row[r] and the
+// input rows in_row[r] (NULL: r).  Up to 8 rows per CTA so that small layers still give every warp a (row, cell) pair;
+// the rows are staged in shared memory when they fit in 48 KB.  Checked by check_ffl / check_td.
+int launch_td_forward_pa(const riab_td_cells* t, long long n_rows, const long long* w_row, const long long* in_row,
+                         const double* pos, float* rates, long long ld, float* prime, cudaStream_t s) {
+  if (n_rows == 0) return 0;
+  const riab_ffl_cells& f = t->ffl;
+  TdFwdPaK k;
+  memset(&k, 0, sizeof(k));
+  int stage_ld = 0;
+  for (int l = 0; l < f.n_inputs; ++l) {
+    const riab_ffl_input& in = f.inputs[l];
+    k.in[l] = in.rows_dev; k.in_ld[l] = in.ld; k.w[l] = t->w_master_dev[l]; k.n_in[l] = in.n_in;
+    k.soff[l] = stage_ld;
+    stage_ld += (in.n_in + 3) / 4 * 4;
+  }
+  k.n_inputs = f.n_inputs; k.n_cells = f.n_cells; k.stage_ld = stage_ld;
+  k.act = ActK{f.activation, f.act[0], f.act[1], f.act[2], f.act[3]};
+  k.bias = f.bias_dev; k.w_row = w_row; k.in_row = in_row; k.pos = pos;
+  k.rates = rates; k.prime = prime; k.ld = ld; k.n_rows = n_rows;
+  constexpr int kStageBytes = 48 * 1024, kWarps = TD_FWD_THREADS / 32;
+  const int rows = std::max(1, kWarps / std::min(f.n_cells, kWarps));
+  const int fit = stage_ld > 0 ? kStageBytes / (stage_ld * 4) : rows;
+  k.rows_per_cta = fit > 0 ? std::min(rows, fit) : rows;
+  const unsigned grid = (unsigned)((n_rows + k.rows_per_cta - 1) / k.rows_per_cta);
+  if (fit > 0) {
+    const size_t smem = (size_t)k.rows_per_cta * stage_ld * 4;
+    k_td_forward_pa<true><<<grid, TD_FWD_THREADS, smem, s>>>(k);
+  } else {
+    k_td_forward_pa<false><<<grid, TD_FWD_THREADS, 0, s>>>(k);
+  }
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;
@@ -2519,7 +2559,8 @@ int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* 
   }
   if (rc || (rc = make_out(out, noise, d.n_cells, dt, ag.id_offset, d.out, d.bound))) return rc;
   if (kind == RIAB_CELLS_BVC) return check_bvc(ek, d.bvc, d.bvc_scratch = out->bvc_scratch, ag.n_agents);
-  if (kind == RIAB_CELLS_TD) return (rc = check_ffl(d.ffl, d.out, ag.n_agents)) ? rc : check_td(d.td, d.out.ld);
+  if (kind == RIAB_CELLS_TD)
+    return (rc = check_ffl(d.ffl, d.out, ag.n_agents, d.td->per_agent_weights == 0)) ? rc : check_td(d.td, d.out.ld);
   if (kind == RIAB_CELLS_NNN) return check_nnn(d.nnn, ag.n_agents);
   return kind == RIAB_CELLS_FFL ? check_ffl(d.ffl, d.out, ag.n_agents) : 0;
 }
@@ -2542,7 +2583,13 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
         return launch_bvc(ek, d.bvc, d.out, ag.pos, n, d.bvc_scratch, d.first_wall, ag.head_direction, s, pipe);
       if (d.kind == RIAB_CELLS_RSN) return launch_rsn(d.rsn, d.place, ek, ag.pos, n, d.out, s);
       if (d.kind == RIAB_CELLS_NNN) return launch_nnn(d.nnn, n, ag.pos, d.out, s);
-      const int rc = launch_ffl(d.ffl, n, ag.pos, d.out, s);
+      int rc;
+      if (d.td != nullptr && d.td->per_agent_weights) {
+        rc = launch_td_forward_pa(d.td, n, nullptr, nullptr, ag.pos, d.out.rates, d.out.ld, d.ffl->prime_dev, s);
+        if (!rc) rc = finish_rows(d.out, d.n_cells, n, s);
+      } else {
+        rc = launch_ffl(d.ffl, n, ag.pos, d.out, s);
+      }
       return (rc || d.kind != RIAB_CELLS_TD) ? rc : launch_td_trace(d.td, n, d.out.rates, s);
     }
     return fail(RIAB_ERR_INVALID, "cells kind %d is launched unfused", d.kind);
@@ -3816,6 +3863,7 @@ int64_t riab_td_scratch_bytes(const riab_td_cells* t, int64_t n_rows) {
     fail(RIAB_ERR_INVALID, "riab_td_scratch_bytes: bad argument");
     return -1;
   }
+  if (t->per_agent_weights) return 0;              // k_td_learn_pa updates the masters in place
   size_t part = 0;
   for (int l = 0; l < t->ffl.n_inputs; ++l) {
     const int n_in = t->ffl.inputs[l].n_in;
@@ -3828,7 +3876,8 @@ int64_t riab_td_scratch_bytes(const riab_td_cells* t, int64_t n_rows) {
 
 int riab_td_learn(const riab_td_cells* t, int64_t n_rows, const void* reward, int32_t reward_mode, float* td_error_out,
                   void* scratch, void* stream) {
-  if (t == nullptr || n_rows < 0 || reward == nullptr || td_error_out == nullptr || scratch == nullptr ||
+  if (t == nullptr || n_rows < 0 || reward == nullptr || td_error_out == nullptr ||
+      (scratch == nullptr && !t->per_agent_weights) ||
       (reward_mode != RIAB_TD_REWARD_SHARED && reward_mode != RIAB_TD_REWARD_ROWS))
     return fail(RIAB_ERR_INVALID, "riab_td_learn: bad argument");
   if (((uintptr_t)scratch) % 16 != 0) return fail(RIAB_ERR_INVALID, "riab_td_learn: scratch must be 16-byte aligned");
@@ -3844,13 +3893,26 @@ int riab_td_learn(const riab_td_cells* t, int64_t n_rows, const void* reward, in
   g.reward_shared = reward_mode == RIAB_TD_REWARD_SHARED ? (const double*)reward : nullptr;
   g.reward_rows = reward_mode == RIAB_TD_REWARD_ROWS ? (const float*)reward : nullptr;
   g.td = td_error_out;
-  g.g = (float*)scratch;
+  g.g = t->per_agent_weights ? nullptr : (float*)scratch;     // the per-agent update forms g from td itself
   g.ld = t->ld; g.ldg = td_g_ld(n); g.n_rows = n_rows; g.n_cells = n;
   g.inv_tau = 1.0 / t->tau;
   const long long ng = n_rows * g.ldg;
   k_td_g<<<(unsigned)((ng + 255) / 256), 256, 0, s>>>(g);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
+  if (t->per_agent_weights) {
+    for (int l = 0; l < f.n_inputs; ++l) {
+      TdLearnPaK k;
+      k.td = td_error_out; k.prime = f.prime_dev; k.e = t->trace_dev[l]; k.w = t->w_master_dev[l];
+      k.ld = t->ld; k.lde = t->trace_ld[l]; k.n_cells = n; k.n_in = f.inputs[l].n_in;
+      k.c_grad = t->dt * t->eta;                      // self.Agent.dt * self.eta
+      k.c_decay = t->eta * t->dt * t->L2;             // self.eta * self.Agent.dt * self.L2
+      k_td_learn_pa<<<(unsigned)n_rows, TD_LEARN_PA_THREADS, 0, s>>>(k);
+      g_launches++;
+      RIAB_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+  }
   double* part = (double*)((char*)scratch + td_g_bytes(n, n_rows));
   for (int l = 0; l < f.n_inputs; ++l) {
     const riab_ffl_input& in = f.inputs[l];
@@ -3879,6 +3941,24 @@ int riab_td_learn(const riab_td_cells* t, int64_t n_rows, const void* reward, in
     RIAB_CUDA_OK(cudaGetLastError());
   }
   return 0;
+}
+
+int riab_td_rates_pa(const riab_td_cells* t, int64_t n_rows, const int64_t* weight_agent_of_row_dev,
+                     const int64_t* input_row_of_row_dev, float* out_dev, int64_t ld_out, void* stream) {
+  if (t == nullptr || n_rows < 0 || (n_rows > 0 && out_dev == nullptr) || ld_out < t->ffl.n_cells)
+    return fail(RIAB_ERR_INVALID, "riab_td_rates_pa: bad argument");
+  if (!t->per_agent_weights) return fail(RIAB_ERR_INVALID, "riab_td_rates_pa: the layer's weights are shared");
+  int rc;
+  OutK out;
+  memset(&out, 0, sizeof(out));
+  out.ld = ld_out;
+  if ((rc = check_ffl(&t->ffl, out, n_rows, false))) return rc;
+  for (int l = 0; l < t->ffl.n_inputs; ++l)
+    if (t->w_master_dev[l] == nullptr || t->ffl.inputs[l].n_in <= 0)
+      return fail(RIAB_ERR_INVALID, "riab_td_rates_pa: input %d has no masters", l);
+  static_assert(sizeof(long long) == sizeof(int64_t), "row maps");
+  return launch_td_forward_pa(t, n_rows, (const long long*)weight_agent_of_row_dev, (const long long*)input_row_of_row_dev,
+                              nullptr, out_dev, ld_out, nullptr, (cudaStream_t)stream);
 }
 
 int riab_td_reset(const riab_td_cells* t, int64_t n_rows, const uint8_t* mask, void* stream) {

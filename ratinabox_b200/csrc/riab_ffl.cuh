@@ -98,8 +98,13 @@ RIAB_DEV float sech2f(float x) {
   return 4.f * e / (d * d);
 }
 
-// utils.activate (utils.py:919-1026) and its derivative, accurate float32; `act` is uniform across the grid.
-RIAB_DEV void ffl_activate(const FflK& k, float x, float& v, float& dv) {
+// utils.activate (utils.py:919-1026) and its derivative, accurate float32; `act` is uniform across the grid.  The one
+// epilogue of every FeedForwardLayer-like contraction (k_ffl here, k_td_forward_pa in riab_td.cuh).
+struct ActK {
+  int act;
+  float p0, p1, p2, p3;
+};
+RIAB_DEV void layer_activate(const ActK& k, float x, float& v, float& dv) {
   switch (k.act) {
     case RIAB_ACT_SIGMOID: {          // p0 max_fr, p1 min_fr, p2 mid_x, p3 beta
       const float z = k.p3 * (x - k.p2);
@@ -133,6 +138,9 @@ RIAB_DEV void ffl_activate(const FflK& k, float x, float& v, float& dv) {
       v = x;
       dv = 1.f;
   }
+}
+RIAB_DEV void ffl_activate(const FflK& k, float x, float& v, float& dv) {
+  layer_activate(ActK{k.act, k.p0, k.p1, k.p2, k.p3}, x, v, dv);
 }
 
 template <int BN>

@@ -17,6 +17,12 @@
 //                dW = dt eta (S / A) - eta dt L2 W applied to the float64 master, and W_hi | W_lo re-split exactly as
 //                riab_ffl_pack does (cvt.rna.tf32 of float32(W), then of the remainder).
 //   k_td_reset   zero fr_prev / deriv / td_error / traces of the masked rows.
+// Per-agent weights (riab_td_cells.per_agent_weights), the masters (A, n, n_in) float64:
+//   k_td_forward_pa  the layer's contraction in place of k_ffl: one warp per (row, cell), the row's inputs staged in
+//                    shared memory, W rows read coalesced in float64, a float64 lane sum then a fixed xor shuffle tree;
+//                    the bias and k_ffl's activation epilogue (layer_activate).  k_finish_rows and k_td_trace follow.
+//   k_td_learn_pa    after k_td_g (td only): W[a] += (dt eta) (td phi')[a, j] e[a, i] - (eta dt L2) W[a], elementwise.
+//   Both stream W once (forward 8 A n n_in bytes, learning 16 A n n_in): bandwidth-bound, no atomics.
 // Every reduction has a fixed order that depends on the shapes only: the stepped API and Agent.run give the same bits,
 // and two identical runs give identical weights.
 #pragma once
@@ -78,7 +84,7 @@ struct TdGK {
   const double* reward_shared;   // (n) or NULL
   const float* reward_rows;      // (A, ld) or NULL
   float* td;                     // (A, ld)
-  float* g;                      // (A, ldg), pads zero
+  float* g;                      // (A, ldg), pads zero; NULL: td only (per-agent weights)
   long long ld, ldg, n_rows;
   int n_cells;
   double inv_tau;
@@ -90,7 +96,7 @@ __global__ void k_td_g(const __grid_constant__ TdGK k) {
   const long long a = idx / k.ldg;
   const int i = (int)(idx - a * k.ldg);
   if (i >= k.n_cells) {
-    k.g[idx] = 0.f;
+    if (k.g) k.g[idx] = 0.f;
     return;
   }
   const long long o = a * k.ld + i;
@@ -98,7 +104,7 @@ __global__ void k_td_g(const __grid_constant__ TdGK k) {
   // the reference's order: reward + dVdt - V / tau
   const double td = (r + (double)k.deriv[o]) - (double)k.fr[o] * k.inv_tau;
   k.td[o] = (float)td;
-  k.g[idx] = (float)(td * (double)k.prime[o]);
+  if (k.g) k.g[idx] = (float)(td * (double)k.prime[o]);
 }
 
 constexpr int TD_KC = 32;            // agents staged per shared-memory round
@@ -332,6 +338,103 @@ __global__ void k_td_reset(const __grid_constant__ TdResetK k) {
       for (long long c = threadIdx.x; c < k.ld; c += blockDim.x) k.rows[b][row * k.ld + c] = 0.f;
   for (int l = 0; l < k.n_inputs; ++l)
     for (long long c = threadIdx.x; c < k.trace_ld[l]; c += blockDim.x) k.trace[l][row * k.trace_ld[l] + c] = 0.f;
+}
+
+// ---- per-agent weights
+struct TdFwdPaK {
+  const float* in[RIAB_FFL_MAX_INPUTS];       // input rows (in_ld floats apart, 16-byte aligned); NULL = zeros
+  long long in_ld[RIAB_FFL_MAX_INPUTS];
+  const double* w[RIAB_FFL_MAX_INPUTS];       // (A, n_cells, n_in[l]) masters
+  int n_in[RIAB_FFL_MAX_INPUTS];
+  int soff[RIAB_FFL_MAX_INPUTS];              // input l's offset in a staged row (floats, a multiple of 4)
+  int n_inputs, n_cells, stage_ld, rows_per_cta;
+  ActK act;
+  const float* bias;                          // (n_cells)
+  const long long* w_row;                     // weight agent of each row, NULL = the row itself
+  const long long* in_row;                    // input row of each row, NULL = the row itself
+  const double* pos;                          // (n_rows, 2): rows whose x is NaN get zeros and keep their prime; or NULL
+  float* rates;                               // (n_rows, ld)
+  float* prime;                               // (n_rows, ld) or NULL
+  long long ld, n_rows;
+};
+
+constexpr int TD_FWD_THREADS = 256;
+
+// STAGED: the CTA's rows_per_cta input rows are copied to shared memory (dynamic, rows_per_cta * stage_ld floats) once and
+// read by every cell's warp; otherwise (rows too long to stage) the warps read them from global memory.  Both sum in the
+// same order.
+template <bool STAGED>
+__global__ void __launch_bounds__(TD_FWD_THREADS) k_td_forward_pa(const __grid_constant__ TdFwdPaK k) {
+  extern __shared__ __align__(16) float td_xs[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r0 = (long long)blockIdx.x * k.rows_per_cta;
+  const int R = (int)min((long long)k.rows_per_cta, k.n_rows - r0);
+  if constexpr (STAGED) {
+    for (int rr = 0; rr < R; ++rr) {
+      const long long ir = k.in_row ? k.in_row[r0 + rr] : r0 + rr;
+      for (int l = 0; l < k.n_inputs; ++l) {
+        float4* dst = reinterpret_cast<float4*>(td_xs + (size_t)rr * k.stage_ld + k.soff[l]);
+        const float4* src = k.in[l] ? reinterpret_cast<const float4*>(k.in[l] + ir * k.in_ld[l]) : nullptr;
+        const int n4 = (k.n_in[l] + 3) >> 2;
+        for (int q = threadIdx.x; q < n4; q += TD_FWD_THREADS) dst[q] = src ? src[q] : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+    __syncthreads();
+  }
+  const int pairs = R * k.n_cells;
+  for (int p = warp; p < pairs; p += TD_FWD_THREADS / 32) {
+    const int rr = p / k.n_cells, j = p - rr * k.n_cells;
+    const long long row = r0 + rr;
+    const long long a = k.w_row ? k.w_row[row] : row;
+    double acc = 0.0;
+    for (int l = 0; l < k.n_inputs; ++l) {
+      if (k.in[l] == nullptr) continue;
+      const int n_in = k.n_in[l];
+      const double* w = k.w[l] + ((size_t)a * k.n_cells + j) * n_in;
+      const float* x;
+      if constexpr (STAGED) x = td_xs + (size_t)rr * k.stage_ld + k.soff[l];
+      else x = k.in[l] + (k.in_row ? k.in_row[row] : row) * k.in_ld[l];
+#pragma unroll 4
+      for (int i = lane; i < n_in; i += 32) acc = fma(__ldcs(w + i), (double)x[i], acc);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc = __dadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
+    if (lane == 0) {
+      const bool nan_row = k.pos != nullptr && isnan(k.pos[2 * row]);
+      float v, dv;
+      layer_activate(k.act, (float)__dadd_rn(acc, (double)k.bias[j]), v, dv);
+      k.rates[row * k.ld + j] = nan_row ? 0.f : v;
+      if (k.prime != nullptr && !nan_row) k.prime[row * k.ld + j] = dv;
+    }
+  }
+}
+
+struct TdLearnPaK {
+  const float* td;        // (A, ld) td_error, written by k_td_g
+  const float* prime;     // (A, ld)
+  const float* e;         // (A, lde) the input's traces
+  double* w;              // (A, n_cells, n_in) masters
+  long long ld, lde;
+  int n_cells, n_in;
+  double c_grad, c_decay; // dt * eta, eta * dt * L2 (the reference's products)
+};
+
+constexpr int TD_LEARN_PA_THREADS = 128;
+
+// one CTA per agent, its n_cells x n_in block in order; dw = (dt eta) (g e) - (eta dt L2) w, w + dw, as the reference
+// evaluates np.outer and its two products, with g = td phi' formed in float64 from the float32 td and phi'
+__global__ void __launch_bounds__(TD_LEARN_PA_THREADS) k_td_learn_pa(const __grid_constant__ TdLearnPaK k) {
+  const long long a = blockIdx.x;
+  const int nw = k.n_cells * k.n_in;
+  double* w = k.w + (size_t)a * nw;
+  const float* e = k.e + a * k.lde;
+  for (int idx = threadIdx.x; idx < nw; idx += TD_LEARN_PA_THREADS) {
+    const int j = idx / k.n_in, i = idx - j * k.n_in;
+    const double g = __dmul_rn((double)k.td[a * k.ld + j], (double)k.prime[a * k.ld + j]);
+    const double wv = __ldcs(w + idx);
+    const double dw = __dsub_rn(__dmul_rn(k.c_grad, __dmul_rn(g, (double)e[i])), __dmul_rn(k.c_decay, wv));
+    __stcs(w + idx, __dadd_rn(wv, dw));
+  }
 }
 
 }  // namespace riab
