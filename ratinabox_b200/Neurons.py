@@ -453,6 +453,11 @@ class PlaceCells(Neurons):
         _lib.check(self._lib.riab_place_pack(_f64p(centres), _f64p(widths), self.n, _f64p(walls), walls.shape[0],
                                              env.los_skip, _f64p(ext), geom, C.byref(c),
                                              host.ctypes.data_as(_lib.c_float_p)))
+        if geom == _lib.WALL_GEOMETRIES["geodesic"] and n_inner == 1 and c.ep_valid == 0:
+            # the reference reduces the detours via the wall's ends inside the box with np.amin, which raises on an
+            # empty list at every rate evaluation (Environment.py:769-773)
+            raise ValueError("zero-size array to reduction operation minimum which has no identity: geodesic distances "
+                             "need an end of the additional wall strictly inside the environment")
         self._packed = self._upload(host)
         self._centres_dev = self._upload(centres)
         c.n_cells, c.description, c.wall_geometry = self.n, _lib.PC_DESCRIPTIONS[self.description], geom
@@ -460,6 +465,9 @@ class PlaceCells(Neurons):
         c.top_hat_width = float(self.widths) if np.isscalar(self.widths) else float(np.asarray(self.widths).reshape(-1)[0])
         c.packed_dev, c.centres_dev = self._packed.data_ptr(), self._centres_dev.data_ptr()
         return c
+
+    def _check_run(self):
+        self._cells()                   # _pack's geodesic check raises before Agent.run stages anything
 
     def _rates_from_positions(self, pos_dev, n_pos, out):
         ag = self.Agent

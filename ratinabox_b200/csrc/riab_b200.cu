@@ -365,12 +365,13 @@ __device__ __forceinline__ void finish4(float (&o)[4], const OutK& out, const Ta
 // ---------------------------------------------------------------------------
 // Cell-type policies for the step kernel.
 // COMP: the compensated direct form (PlaceConst::comp, riab_place.cuh): kernels of their own, chosen by the host, so the
-// expanded and geodesic kernels keep their code and registers.
-template <int WI, int DESC, bool COMP = false>
+// expanded kernels keep their code and registers.  GEO: the geodesic kernel (one inner wall, run-time profile, COMP), whose
+// record carries the agent -> wall-end distances as well.
+template <int WI, int DESC, bool COMP = false, bool GEO = false>
 struct PlacePolicy {
   using Const = PlaceConst;
   using Regs = PlaceCellRegs<WI>;
-  static constexpr int REC = place_rec(WI);
+  static constexpr int REC = place_rec(WI, GEO);
   static constexpr bool LIGHT = (WI == 0) && (DESC >= 0) && !COMP;   // few instructions per rate: HBM-bound consumers
   // rates lie in [min_fr, max_fr], so the thinned spike stream applies, but it measured slower for place cells: the
   // Euclidean Gaussian loop is HBM-bound and hides the dense stream's instructions under its stores, the line-of-sight
@@ -383,13 +384,13 @@ struct PlacePolicy {
   }
   static __device__ __forceinline__ void record(float* rec, long long, double px, double py, double, double, double, double, double, double,
                                                 const double* s_walls, const double* aux, const Const& c, const EnvK& env) {
-    place_agent_record<WI, COMP>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, c.geometry, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
+    place_agent_record<WI, COMP, GEO>(rec, px, py, s_walls + 4 * c.wall0, aux, WI > 0 ? c.n_inner : 0, env.cxm, env.cym, c.band, c.expanded, c.kx, c.fold ? c.lspan : 0.f);
   }
-  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI, COMP>(r, c, cell0); }
+  static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) { place_load_cells<WI, COMP, GEO>(r, c, cell0); }
   template <bool DEFER, int EXP = -1>
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int cell0,
                                                 const float* rec, uint32_t inner_s, bool& unsure) {
-    place_rates4<WI, DESC, DEFER, EXP, COMP>(o, r, c, cell0, rec, inner_s, unsure);
+    place_rates4<WI, DESC, DEFER, EXP, COMP, GEO>(o, r, c, cell0, rec, inner_s, unsure);
   }
   // 0: direct form, 1: expanded exponent, 2: expanded with the [0, max_fr] scale folded into the exponent
   static __device__ __forceinline__ int expanded(const Const& c) {
@@ -512,12 +513,12 @@ struct AvcPolicy {
 // PhasePrecessingPlaceCells: PlacePolicy's record, cells and rates (direct exponent form), times the theta modulation
 // factor of riab_pppc.cuh.  MODE 0 reads the rows' velocities from Const::vel (given_dir: the one given vector stands for
 // every kinematic input).
-template <int WI, int DESC, bool COMP = false>
+template <int WI, int DESC, bool COMP = false, bool GEO = false>
 struct PppcPolicy {
-  using Place = PlacePolicy<WI, DESC, COMP>;
+  using Place = PlacePolicy<WI, DESC, COMP, GEO>;
   using Const = PppcConst;
   using Regs = PppcCellRegs<WI>;
-  static constexpr int REC = pppc_rec(WI);
+  static constexpr int REC = pppc_rec(WI, GEO);
   static constexpr bool LIGHT = false;    // ~10 more instructions per rate and 12 more cell registers than PlacePolicy
   static constexpr bool THIN = false;     // the factor has no a-priori bound below M max_fr: dense spike stream
   static constexpr bool POSITIONAL = true;
@@ -531,7 +532,7 @@ struct PppcPolicy {
                                                 double vx, double vy, double mvx, double mvy, const double* s_walls,
                                                 const double* aux, const Const& c, const EnvK& env) {
     Place::record(rec, i, px, py, hdx, hdy, vx, vy, mvx, mvy, s_walls, aux, c, env);
-    pppc_direction_record(rec + pppc_dir(WI), px, py, vx, vy, env.cxm, env.cym);
+    pppc_direction_record(rec + pppc_dir(WI, GEO), px, py, vx, vy, env.cxm, env.cym);
   }
   static __device__ __forceinline__ void load(Regs& r, const Const& c, int cell0) {
     Place::load(r.p, c, cell0);
@@ -541,7 +542,7 @@ struct PppcPolicy {
   static __device__ __forceinline__ void rates4(float (&o)[4], const Regs& r, const Const& c, int cell0,
                                                 const float* rec, uint32_t inner_s, bool& unsure) {
     Place::template rates4<DEFER, 0>(o, r.p, c, cell0, rec, inner_s, unsure);
-    pppc_modulate4<WI>(o, r, c, rec + pppc_dir(WI));
+    pppc_modulate4<WI>(o, r, c, rec + pppc_dir(WI, GEO));
   }
   static __device__ __forceinline__ int expanded(const Const&) { return 0; }
   static __device__ __forceinline__ int wall0(const Const& c) { return c.wall0; }
@@ -1170,17 +1171,8 @@ __device__ __forceinline__ double onehot_exact_dist(const PlaceConst& c, int cel
   }
   const double d = dsqrt(ex * ex + ey * ey).v;
   if (!blocked) return d;
-  if (c.geometry == RIAB_GEOM_GEODESIC) {
-    double via = INFINITY;
-    for (int e = 0; e < 2; ++e) {
-      if (!((c.ep_valid >> e) & 1)) continue;
-      const D wx(inner64[2 * e]), wy(inner64[2 * e + 1]);
-      const D ax = D(cx) - wx, ay = D(cy) - wy, bx = wx - D(px), by = wy - D(py);
-      const double v = (dsqrt(ax * ax + ay * ay) + dsqrt(bx * bx + by * by)).v;
-      via = fmin(via, v);
-    }
-    return via;
-  }
+  if (c.geometry == RIAB_GEOM_GEODESIC)
+    return geodesic_detour_exact(cx, cy, px, py, inner64[0], inner64[1], inner64[2], inner64[3], c.ep_valid);
   return 1000.0;
 }
 
@@ -1716,6 +1708,9 @@ int make_place(const riab_place_cells* pc, const EnvK& env, PlaceConst& c) {
     if (pc->centres_dev == nullptr) return fail(RIAB_ERR_INVALID, "centres_dev NULL");
     if (pc->wall_geometry == RIAB_GEOM_GEODESIC && n_inner > 1)
       return fail(RIAB_ERR_INVALID, "geodesic geometry is only defined with one additional wall (Environment.py:736-739)");
+    // the reference's np.amin over the detours via the ends inside the box has nothing to reduce (Environment.py:769-773)
+    if (pc->wall_geometry == RIAB_GEOM_GEODESIC && n_inner == 1 && pc->ep_valid == 0)
+      return fail(RIAB_ERR_INVALID, "geodesic geometry needs an end of the additional wall strictly inside the box");
   }
   if ((pc->description == RIAB_PC_TOP_HAT || pc->description == RIAB_PC_ONE_HOT) && pc->centres_dev == nullptr)
     return fail(RIAB_ERR_INVALID, "centres_dev NULL");
@@ -1737,8 +1732,9 @@ int make_place(const riab_place_cells* pc, const EnvK& env, PlaceConst& c) {
   c.lspan = c.fold ? log2f(c.span) : 0.f;
   // The direct form rounds p' and c' to float32 separately, |d_f - d| ~ 2^-24 (|p'| + |c'|): a relative rate error of
   // ~ d |d_f - d| / w^2, 2.5e-5 at 3.7 w with w = 0.05 in a 10 m box and near 1e-5 already at w = 0.05 in the unit box.
-  // Every direct-form launch without geodesic detours (which use ep0 / ep1) therefore takes the compensated kernels.
-  c.comp = (!c.expanded && pc->wall_geometry != RIAB_GEOM_GEODESIC && pc->description != RIAB_PC_ONE_HOT) ? 1 : 0;
+  // Every direct-form launch therefore takes the compensated kernels, geodesic included: its record holds the agent ->
+  // wall-end distances in a block of their own (place_geo), so ep0 / ep1 carry the residuals there too.
+  c.comp = (!c.expanded && pc->description != RIAB_PC_ONE_HOT) ? 1 : 0;
   c.periodic = env.periodic; c.scale = env.scale; c.scale_f = (float)env.scale; c.half_f = (float)(env.scale / 2);
   c.scale_lo = (float)(env.scale - (double)c.scale_f);
   {
@@ -1855,7 +1851,7 @@ int make_pppc(const riab_pppc_cells* pc, const EnvK& env, const double* vel, Ppp
     return fail(RIAB_ERR_INVALID, "phase precessing place cells: theta_freq %g, sigma %g, precess_fraction %g, t %g",
                 pc->theta_freq, pc->sigma, pc->precess_fraction, pc->t);
   c.expanded = 0; c.fold = 0; c.lspan = 0.f;                          // the direct form of the DESC = -1 kernels
-  c.comp = (pc->place.wall_geometry != RIAB_GEOM_GEODESIC) ? 1 : 0;  // compensated (make_place)
+  c.comp = 1;                                                          // compensated (make_place)
   const double period = 1.0 / pc->theta_freq;
   double r = fmod(pc->t, period);                                      // Python's t % period: the sign of the divisor
   if (r != 0.0 && ((r < 0.0) != (period < 0.0))) r += period;
@@ -1969,20 +1965,27 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   return 0;
 }
 
-// A Place-like policy (PlacePolicy, PppcPolicy) for pc's compensated-sum switch and inner walls (compile-time bound 0, 1,
-// 2, 4 or 8); called with COMP = false, it first picks COMP from pc.comp
-template <template <int, int, bool> class Pol, int MODE, int DESC, bool COMP = false, class C>
+// A Place-like policy (PlacePolicy, PppcPolicy) for pc's geometry, compensated-sum switch and inner walls (compile-time
+// bound 0, 1, 2, 4 or 8); called with COMP = false, it first picks COMP from pc.comp.  Geodesic has one inner wall
+// (make_place) and the run-time profile switch; its kernel and every other DESC = -1 kernel take the compensated form.
+template <template <int, int, bool, bool> class Pol, int MODE, int DESC, bool COMP = false, class C>
 int launch_walls(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const C& pc,
                  const OutK& out, const double* pos_in, long long n_rows, cudaStream_t s, const RunK* run) {
-  if constexpr (!COMP) {
-    if (pc.comp) return launch_walls<Pol, MODE, DESC, true>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  if constexpr (DESC < 0 && !COMP) {
+    if (pc.geometry == RIAB_GEOM_GEODESIC)
+      return launch_tile<Pol<1, DESC, true, true>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    return launch_walls<Pol, MODE, DESC, true>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+  } else {
+    if constexpr (!COMP) {
+      if (pc.comp) return launch_walls<Pol, MODE, DESC, true>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    }
+    const int wi = pc.n_inner;
+    if (wi == 0) return launch_tile<Pol<0, DESC, COMP, false>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi == 1) return launch_tile<Pol<1, DESC, COMP, false>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi == 2) return launch_tile<Pol<2, DESC, COMP, false>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    if (wi <= 4) return launch_tile<Pol<4, DESC, COMP, false>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
+    return launch_tile<Pol<8, DESC, COMP, false>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
   }
-  const int wi = pc.n_inner;
-  if (wi == 0) return launch_tile<Pol<0, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi == 1) return launch_tile<Pol<1, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi == 2) return launch_tile<Pol<2, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  if (wi <= 4) return launch_tile<Pol<4, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
-  return launch_tile<Pol<8, DESC, COMP>, MODE>(env, ag, mp, io, pc, out, pos_in, n_rows, s, run);
 }
 
 int launch_onehot(const EnvK& env, const PlaceConst& pc, const OutK& out, const double* pos, long long n_rows,

@@ -30,9 +30,12 @@ constexpr int PLACE_MAX_WI = 8;      // inner walls held in registers
 // with s = sign(f_p): multiplied by the cell's SIGNED f_c these give |f_c| t_p/|f_p| etc. exactly when centre and agent
 // lie on opposite sides of the wall's line (the only case in which X and Y matter), with no |.| on the cell side.
 constexpr int PLACE_WALL0 = 4;                               // float index of wall 0's float4
-// record of a policy with WI inner-wall slots: [px, py, ep0, ep1] [wall float4] x WI [float64 px, py]
+// record of a policy with WI inner-wall slots: [px, py, ep0, ep1] [wall float4] x WI [float64 px, py] and, for geodesic
+// kernels (GEO), [|e0 - p|, |e1 - p|, 0, 0]: the agent -> wall-end distances of the detour, so that ep0 / ep1 stay free
+// for the compensated direct form
 constexpr int place_pos64(int wi) { return PLACE_WALL0 + 4 * wi; }   // float index of the float64 position
-constexpr int place_rec(int wi) { return place_pos64(wi) + 4; }      // 16 floats = 64 B per agent with two inner walls
+constexpr int place_geo(int wi) { return place_pos64(wi) + 4; }      // float index of the wall-end distances (GEO)
+constexpr int place_rec(int wi, bool geo = false) { return place_pos64(wi) + (geo ? 8 : 4); }   // 16 floats with two walls
 constexpr float PLACE_PEN = 1.2676506002282294e30f;          // 2^100: pen * PLACE_PEN is >= 1e24 for every certain blocked pair
 constexpr float PLACE_QSCALE = 1048576.0f;                   // 2^20: q' = f_c * (-f_p * 2^20) never enters the band by magnitude
 
@@ -60,6 +63,20 @@ RIAB_DEV bool los_blocked_exact(double cx, double cy, double px, double py, cons
   return los_blocked_exact(cx, cy, px, py, w[0], w[1], w[2], w[3]);
 }
 
+// The reference's float64 geodesic detour centre -> wall end -> pos, the minimum over the ends inside the box
+// (ep_valid bit e: end e at (w[2e], w[2e+1])), Environment.py:745-773; INFINITY when no end is inside.
+RIAB_DEV double geodesic_detour_exact(double cx, double cy, double px, double py, double w0, double w1, double w2,
+                                      double w3, int ep_valid) {
+  double via = INFINITY;
+  for (int e = 0; e < 2; ++e) {
+    if (!((ep_valid >> e) & 1)) continue;
+    const D wx(e ? w2 : w0), wy(e ? w3 : w1);
+    const D ax = D(cx) - wx, ay = D(cy) - wy, bx = wx - D(px), by = wy - D(py);
+    via = fmin(via, (dsqrt(ax * ax + ay * ay) + dsqrt(bx * bx + by * by)).v);
+  }
+  return via;
+}
+
 // Per-agent record for the rate phase, from the float64 position.
 // inner = walls + 4*n_boundary (float64 endpoints), cxm/cym = box centre.
 // Per-CTA wall invariants of the agent records (shared memory, 2 doubles per inner wall): 1 / |s| and 1 / |s|^2, so that a
@@ -75,18 +92,22 @@ RIAB_DEV void place_wall_invariants(double* __restrict__ aux, const double* __re
 }
 
 // COMP: the compensated direct form -- ep0 / ep1 carry the float32 residuals of the centred position (unused slots there:
-// neither the expanded form nor geodesic detours take COMP).
-template <int WI, bool COMP = false>
+// the expanded form does not take COMP).  GEO: the geodesic kernels' wall-end distances at place_geo(WI).
+template <int WI, bool COMP = false, bool GEO = false>
 RIAB_DEV void place_agent_record(float* __restrict__ rec, double px, double py, const double* __restrict__ inner,
                                  const double* __restrict__ aux,
-                                 int n_inner, int geometry, double cxm, double cym, float band, int expanded, float kx,
+                                 int n_inner, double cxm, double cym, float band, int expanded, float kx,
                                  float lfold /* log2(span) when the scale is folded into the exponent, else 0 */) {
   float ep0 = 0.f, ep1 = 0.f;
-  if (geometry == RIAB_GEOM_GEODESIC && n_inner >= 1) {
-    // utils.get_distances_between(wall_edge, pos2)  (Environment.py:749-751)
-    const double e0x = inner[0] - px, e0y = inner[1] - py, e1x = inner[2] - px, e1y = inner[3] - py;
-    ep0 = (float)sqrt(e0x * e0x + e0y * e0y);
-    ep1 = (float)sqrt(e1x * e1x + e1y * e1y);
+  if (GEO) {
+    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (n_inner >= 1) {
+      // utils.get_distances_between(wall_edge, pos2)  (Environment.py:749-751)
+      const double e0x = inner[0] - px, e0y = inner[1] - py, e1x = inner[2] - px, e1y = inner[3] - py;
+      g.x = (float)sqrt(e0x * e0x + e0y * e0y);
+      g.y = (float)sqrt(e1x * e1x + e1y * e1y);
+    }
+    *reinterpret_cast<float4*>(rec + place_geo(WI)) = g;
   }
   const float pxf = (float)(px - cxm), pyf = (float)(py - cym);
   if (expanded) ep0 = (float)((double)kx * ((double)pxf * pxf + (double)pyf * pyf) + (double)lfold);   // -k |p|^2 [+ log2 span]
@@ -125,7 +146,7 @@ struct PlaceConst {                  // uniform per launch
   const float* packed;               // device
   const double* centres64;           // device (N,2)
   int periodic;                      // wrap centre->agent vectors (Environment.py:670-675)
-  int comp;                          // direct form, not geodesic: the host launches the COMP kernels (make_place)
+  int comp;                          // direct form: the host launches the COMP kernels (make_place)
   float scale_f, half_f;
   double scale;
   double cxm, cym;
@@ -143,7 +164,7 @@ struct PlaceCellRegs {
   float cxl[4], cyl[4];              // COMP only: residuals of the centred centres
 };
 
-template <int WI, bool COMP = false>
+template <int WI, bool COMP = false, bool GEO = false>
 RIAB_DEV void place_load_cells(PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0) {
   const float* base = c.packed;
   const int np = c.n_pad;
@@ -168,7 +189,7 @@ RIAB_DEV void place_load_cells(PlaceCellRegs<WI>& r, const PlaceConst& c, int ce
 #pragma unroll
     for (int i = 0; i < 4; ++i) r.tq[j][i] = 1.f - r.tc[j][i];
   }
-  if (WI > 0 && c.geometry == RIAB_GEOM_GEODESIC) {
+  if (GEO) {
     ldv(r.ce0, base + (4 + 2 * c.n_inner) * np + cell0);
     ldv(r.ce1, base + (5 + 2 * c.n_inner) * np + cell0);
   }
@@ -237,7 +258,8 @@ RIAB_DEV float periodic_comp(float p, float cc, float lo, const PlaceConst& c) {
 //   EXP     : 1 = the expanded Gaussian form is known to be on (no branch), 0 = known off, -1 = test c.expanded
 //   COMP    : direct form with the float32 residuals of p' (record ep0 / ep1) and c' (cxl / cyl):
 //             dx = (px - cx) + (pxl - cxl), so |p'| and |c'| no longer limit the accuracy of d (PlaceConst::comp)
-template <int WI, int DESC, bool DEFER, int EXP = -1, bool COMP = false>
+//   GEO     : geodesic detours for blocked pairs (one inner wall, DESC = -1, the record's place_geo block)
+template <int WI, int DESC, bool DEFER, int EXP = -1, bool COMP = false, bool GEO = false>
 RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const PlaceConst& c, int cell0,
                            const float* __restrict__ rec, uint32_t inner_s, bool& unsure_io) {
   const float4 r0 = *reinterpret_cast<const float4*>(rec);          // px, py, ep0 | -k|p|^2, ep1
@@ -335,7 +357,7 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
   float dd[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) dd[i] = (WI > 0) ? fmaf(pen[i], PLACE_PEN, d2[i]) : d2[i];
-  const bool geodesic = (DESC < 0) && (WI > 0) && (c.geometry == RIAB_GEOM_GEODESIC);
+  constexpr bool geodesic = GEO && (DESC < 0) && (WI > 0);
   const int desc = (DESC >= 0) ? DESC : c.desc;
   if (desc != RIAB_PC_TOP_HAT && !geodesic) {
 #pragma unroll
@@ -343,7 +365,7 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
       out[i] = fmaf(place_profile<DESC>(dd[i], r.k[i], c.desc), c.span, c.min_fr);   // Neurons.py:978-980
     return;
   }
-  const float2 ep = make_float2(r0.z, r0.w);
+  const float4 ep = geodesic ? *reinterpret_cast<const float4*>(rec + place_geo(WI)) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const bool blocked = (WI > 0) && (dd[i] != d2[i]);
@@ -357,18 +379,26 @@ RIAB_DEV void place_rates4(float (&out)[4], const PlaceCellRegs<WI>& r, const Pl
     }
     float v;
     if (desc == RIAB_PC_TOP_HAT) {
-      // Neurons.py:975-976: 1*(dist < widths) with the scalar `widths`
+      // Neurons.py:975-976: 1*(dist < widths) with the scalar `widths`.  A line-of-sight blocked pair has dv >= 1e24;
+      // a geodesic detour's dv = (ce + ep)^2 carries three float32 roundings of the sum and one of the square, under
+      // 5e-7 relative, well inside top_hat_band (>= 4e-6 w^2): both forms take the float64 decision near the edge.
       bool in = dv < c.top_hat_w2;
-      if (fabsf(dv - c.top_hat_w2) < c.top_hat_band && !blocked) {
+      if (fabsf(dv - c.top_hat_w2) < c.top_hat_band && (geodesic || !blocked)) {
         const int cell = cell0 + i;
         if (cell < c.n_cells) {
           const double2 p64 = *reinterpret_cast<const double2*>(rec + place_pos64(WI));
-          D ex = D(c.centres64[2 * cell]) - D(p64.x), ey = D(c.centres64[2 * cell + 1]) - D(p64.y);
-          if (c.periodic) {
-            if (fabs(ex.v) > c.scale / 2) ex = D(-copysign(1.0, ex.v)) * (D(c.scale) - D(fabs(ex.v)));
-            if (fabs(ey.v) > c.scale / 2) ey = D(-copysign(1.0, ey.v)) * (D(c.scale) - D(fabs(ey.v)));
+          const double cx = c.centres64[2 * cell], cy = c.centres64[2 * cell + 1];
+          if (geodesic && blocked) {
+            in = geodesic_detour_exact(cx, cy, p64.x, p64.y, lds_f64(inner_s), lds_f64(inner_s + 8u),
+                                       lds_f64(inner_s + 16u), lds_f64(inner_s + 24u), c.ep_valid) < c.top_hat_w;
+          } else {
+            D ex = D(cx) - D(p64.x), ey = D(cy) - D(p64.y);
+            if (c.periodic) {
+              if (fabs(ex.v) > c.scale / 2) ex = D(-copysign(1.0, ex.v)) * (D(c.scale) - D(fabs(ex.v)));
+              if (fabs(ey.v) > c.scale / 2) ey = D(-copysign(1.0, ey.v)) * (D(c.scale) - D(fabs(ey.v)));
+            }
+            in = dsqrt(ex * ex + ey * ey).v < c.top_hat_w;
           }
-          in = dsqrt(ex * ex + ey * ey).v < c.top_hat_w;
         }
       }
       v = in ? 1.f : 0.f;

@@ -19,8 +19,8 @@
 
 namespace riab {
 
-constexpr int pppc_dir(int wi) { return place_rec(wi); }     // float index of (d_x, d_y, p.d, 0) in the record
-constexpr int pppc_rec(int wi) { return place_rec(wi) + 4; }
+constexpr int pppc_dir(int wi, bool geo) { return place_rec(wi, geo); }   // float index of (d_x, d_y, p.d, 0) in the record
+constexpr int pppc_rec(int wi, bool geo) { return place_rec(wi, geo) + 4; }
 
 struct PppcConst : PlaceConst {      // uniform per launch; the PlaceCells constants in their direct form (expanded = fold = 0)
   float u;                          // (pi - phi) / 2 pi of the launch's clock

@@ -51,9 +51,10 @@ constexpr int rsn_threads() { return 128 * CWG + 32; }
 
 template <int WI, int DESC, int BN, int CWG>
 __global__ void __launch_bounds__(rsn_threads<CWG>(), 1) k_rsn(const __grid_constant__ RsnK k) {
+  constexpr bool GEO = DESC < 0;      // the run-time profile kernel is the geodesic one (launch_rsn): GEO agent records
   constexpr int BM = 64 * CWG, CONSUMER_WARPS = 4 * CWG;
   constexpr int T_BYTES = BN * FFL_BK * 4;
-  constexpr int REC = place_rec(WI);
+  constexpr int REC = place_rec(WI, GEO);
   extern __shared__ uint8_t rsn_smem_raw[];
   __shared__ __align__(8) uint64_t full[RSN_STAGES], empty[RSN_STAGES];
   __shared__ __align__(16) float s_rec[BM * REC];
@@ -77,8 +78,8 @@ __global__ void __launch_bounds__(rsn_threads<CWG>(), 1) k_rsn(const __grid_cons
   if (threadIdx.x < BM) {                                      // one record per agent row of the tile
     const long long row = m0 + threadIdx.x;
     const double px = row < k.n_rows ? k.pos[2 * row] : pc.cxm, py = row < k.n_rows ? k.pos[2 * row + 1] : pc.cym;
-    place_agent_record<WI>(s_rec + threadIdx.x * REC, px, py, s_inner, s_aux, n_inner, pc.geometry, pc.cxm, pc.cym,
-                           pc.band, 0, 0.f, 0.f);
+    place_agent_record<WI, false, GEO>(s_rec + threadIdx.x * REC, px, py, s_inner, s_aux, n_inner, pc.cxm, pc.cym,
+                                       pc.band, 0, 0.f, 0.f);
   }
   __syncthreads();
 
@@ -115,11 +116,11 @@ __global__ void __launch_bounds__(rsn_threads<CWG>(), 1) k_rsn(const __grid_cons
     for (int run = 0; run < 2; ++run) {                            // packed points 8 q + 4 run .. + 3: k8 = 2 run, 2 run + 1
       const int cell0 = it * FFL_BK + 8 * q + 4 * run;
       PlaceCellRegs<WI> r;
-      place_load_cells<WI>(r, pc, cell0);
+      place_load_cells<WI, false, GEO>(r, pc, cell0);
       float v0[4], v1[4];
       bool unsure = false;
-      place_rates4<WI, DESC, false, 0>(v0, r, pc, cell0, rec0, inner_s, unsure);
-      place_rates4<WI, DESC, false, 0>(v1, r, pc, cell0, rec1, inner_s, unsure);
+      place_rates4<WI, DESC, false, 0, false, GEO>(v0, r, pc, cell0, rec0, inner_s, unsure);
+      place_rates4<WI, DESC, false, 0, false, GEO>(v1, r, pc, cell0, rec1, inner_s, unsure);
       if (tail) {
 #pragma unroll
         for (int i = 0; i < 4; ++i)

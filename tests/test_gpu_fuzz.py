@@ -1,7 +1,7 @@
 """Seeded differential fuzzing of the CUDA path against the oracle: random wall layouts (0..7 inner walls, some
 touching the boundary or each other), random Agent parameters, random cell populations; teacher-forced steps
 (injected normals, zero jitter) so positions are comparable to 1e-12 step by step, then every cell type's rates at the
-reached positions.  GPU only."""
+reached positions, and geodesic PlaceCells there in a box holding only the first wall.  GPU only."""
 import numpy as np
 import pytest
 
@@ -95,6 +95,21 @@ def test_random_environment_motion_and_rates(seed):
         ref = O.place_cells_get_state(env, P.place_cell_centres, P.place_cell_widths, pos, rng, desc, geom,
                                       scalar_width=(None if per_cell else 0.18)).T
         assert np.abs(P.get_state(evaluate_at=None, pos=pos).T - ref).max() <= 1e-5, (seed, desc, geom)
+    if walls:
+        # geodesic PlaceCells in a box holding only the seed's first wall (from the boundary or free-standing)
+        rg = np.random.RandomState(2000 + seed)
+        E1 = rb.Environment()
+        E1.add_wall(walls[0])
+        env1 = O.OracleEnvironment(walls=walls[:1])
+        desc = ["gaussian", "gaussian_threshold", "diff_of_gaussians", "top_hat", "one_hot"][rg.randint(5)]
+        per_cell = rg.randint(2) == 1 and desc not in ("top_hat", "one_hot")
+        w = float(rg.uniform(0.08, 0.3))
+        widths = rg.uniform(0.08, 0.3, size=40) if per_cell else w
+        P = rb.PlaceCells(rb.Agent(E1, {"n_agents": 1}), {"n": 40, "description": desc, "widths": widths})
+        assert P.wall_geometry == "geodesic" and P._effective_geometry() == "geodesic"
+        ref = O.place_cells_get_state(env1, P.place_cell_centres, P.place_cell_widths, pos, rng, desc, "geodesic",
+                                      scalar_width=(None if per_cell else w)).T
+        assert np.abs(P.get_state(evaluate_at=None, pos=pos).T - ref).max() <= 1e-5, (seed, desc, "geodesic", walls[0])
     G = rb.GridCells(Ag, {"n": 20})
     assert np.abs(G.get_state(evaluate_at=None, pos=pos) - O.grid_cells_get_state(G.gridscales, G.phase_offsets, G.w, pos)).max() <= 1e-5
     B = rb.BoundaryVectorCells(Ag, {"n": 12})

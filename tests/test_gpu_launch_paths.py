@@ -33,6 +33,7 @@ WALLS = {
     3: BOX_WALLS + [[[0.0, 0.75], [0.2, 0.75]]],
     7: [[[k / 8, 0.0], [k / 8, 0.6]] if k % 2 else [[k / 8, 1.0], [k / 8, 0.4]] for k in range(1, 8)],
     "aspect2": [[[0.6, 0.0], [0.6, 0.5]], [[1.4, 1.0], [1.4, 0.5]]],
+    "free": [[[0.5, 0.2], [0.5, 0.8]]],             # both ends inside the box
 }
 
 
@@ -57,7 +58,8 @@ def batch(kind, n_cells):
 
 
 # name: (kind, n_cells, batch, W's path, extra parameters)
-#   walls / aspect / desc / widths / min_fr / max_fr / dt: the set-up;  steps, pre: compared steps after `pre` stepped ones;
+#   walls / geom / aspect / desc / widths / min_fr / max_fr / dt: the set-up (geom: the place cells' wall_geometry,
+#   line_of_sight unless given);  steps, pre: compared steps after `pre` stepped ones;
 #   rows / agent_rows: history_bytes_limit of the population / Agent in rows (default: the library's limits);
 #   off: id_offset;  spikes / history: save_spikes / save_history
 CASES = {
@@ -75,6 +77,15 @@ CASES = {
     "place_2048_one_group": ("place", 2048, "rounds", "whole", dict(walls=2, steps=4)),
     "place_even_offset": ("place", 512, "odd", "whole", dict(walls=2, off=64, steps=10)),
     "place_odd_offset": ("place", 512, "odd", "step", dict(walls=2, off=33, steps=10)),
+    # geodesic (one inner wall): the compensated direct form with the wall-end block of the agent record
+    "place_geodesic_end_on_boundary": ("place", 512, "odd", "whole", dict(walls=1, geom="geodesic", steps=10, pre=2,
+                                                                          rows=3)),
+    "place_geodesic_free_wall_dog": ("place", 512, "one_slot", "whole", dict(walls="free", geom="geodesic",
+                                                                            desc="diff_of_gaussians", steps=8)),
+    "place_geodesic_top_hat": ("place", 512, "odd", "whole", dict(walls="free", geom="geodesic", desc="top_hat",
+                                                                  widths=0.3, steps=10)),
+    "place_geodesic_rounds": ("place", 388, "rounds", "whole", dict(walls=1, geom="geodesic", widths="per_cell",
+                                                                    min_fr=0.1, steps=6)),
     "place_no_history": ("place", 512, "one_slot", "whole", dict(walls=2, history=False, steps=10)),
     "place_256_cells": ("place", 256, "odd", "step", dict(walls=2, steps=8)),
     "place_390_cells": ("place", 390, "odd", "step", dict(walls=0, steps=8)),
@@ -104,7 +115,7 @@ def _cell_params(kind, n, p):
         if isinstance(widths, str):
             widths = rs.uniform(0.1, 0.25, n)
         return {"n": n, "place_cell_centres": np.stack((rs.uniform(0, aspect, n), rs.uniform(0, 1, n)), axis=1),
-                "widths": widths, "description": p.get("desc", "gaussian"), "wall_geometry": "line_of_sight",
+                "widths": widths, "description": p.get("desc", "gaussian"), "wall_geometry": p.get("geom", "line_of_sight"),
                 "min_fr": p.get("min_fr", 0.0), "max_fr": p.get("max_fr", 1.0)}
     return {"gridscale": rs.uniform(0.2, 1.0, n), "orientation": rs.uniform(0, np.pi / 3, n),
             "phase_offset": rs.uniform(0, 2 * np.pi, (n, 2)), "description": p.get("desc", "rectified_cosines"),
@@ -274,13 +285,15 @@ def test_whole_run_equals_per_step_paths(name, monkeypatch):
     fr = W["firingrate"][sample]
     span = p.get("max_fr", 1.0) - p.get("min_fr", 0.0)
     if kind == "place":
-        geom = "euclidean" if p.get("walls", 0) == 0 else "line_of_sight"
+        geom = "euclidean" if p.get("walls", 0) == 0 else p.get("geom", "line_of_sight")
+        assert Ns._effective_geometry() == geom
         desc = p.get("desc", "gaussian")
         scalar = Ns.widths if np.isscalar(Ns.widths) else None
         ref = O.place_cells_get_state(env, Ns.place_cell_centres, Ns.place_cell_widths, pos, O.TapeRNG(), desc, geom,
                                       p.get("min_fr", 0.0), p.get("max_fr", 1.0), scalar_width=scalar).T
-        if geom == "line_of_sight":
-            blocked = O.distances_accounting_for_environment(env, Ns.place_cell_centres, pos, geom, O.TapeRNG()).T == 1000
+        if geom != "euclidean":
+            blocked = O.distances_accounting_for_environment(env, Ns.place_cell_centres, pos, "line_of_sight",
+                                                             O.TapeRNG()).T == 1000
             assert blocked.mean() > 0.02, blocked.mean()        # the wall shadows are exercised
     else:
         ref = O.grid_cells_get_state(Ns.gridscales, Ns.phase_offsets, Ns.w, pos, p.get("desc", "rectified_cosines"),

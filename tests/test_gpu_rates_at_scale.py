@@ -29,6 +29,8 @@ from ratinabox_b200.contribs import SpatialGoalEnvironment   # noqa: E402
 
 TOL = 1e-5
 C2 = [[[0.3, 0.0], [0.3, 0.5]], [[0.7, 1.0], [0.7, 0.5]]]   # two walls of the unit box, scaled with the box below
+GEO = [[[0.5, 0.2], [0.5, 0.8]]]                            # geodesic: one wall, both ends inside the box
+GEO_END = [[[0.5, 0.0], [0.5, 0.6]]]                        # geodesic: one wall, one end on the boundary
 SHIFT = np.array([1000.0, -500.0])
 LROOM = {"boundary": [[0, 0], [1, 0], [1, 0.5], [0.5, 0.5], [0.5, 1], [0, 1]], "walls": [[[0.25, 0.0], [0.25, 0.3]]]}
 HOLED = {"boundary": [[0, 0], [1, 0], [1, 1], [0, 1]], "holes": [[[0.4, 0.4], [0.6, 0.4], [0.6, 0.6], [0.4, 0.6]]],
@@ -109,13 +111,41 @@ def _agent(E, n=1, seed=3):
     return rb.Agent(E, {"dt": 0.01, "n_agents": n, "seed": seed})
 
 
+def _walls_of(geom):
+    return {"line_of_sight": C2, "geodesic": GEO}.get(geom, ())
+
+
+def _wall_ends(env):
+    """The ends of the one inner wall that lie inside the box (the geodesic detours' corners)."""
+    return [e for e in np.asarray(env.walls[4], dtype=float) if env.contains(e)]
+
+
+def _around_ends(rs, env, r_max, n_r=12, n_a=16, jitter=True):
+    """Rings of radius (0, r_max] around the inner wall's ends inside the box, clipped to the box: both sides of the wall
+    near an end, where blocked pairs have short detours."""
+    P = []
+    for e in _wall_ends(env):
+        r = np.linspace(0, r_max, n_r + 1)[1:, None]
+        a = np.linspace(0, 2 * np.pi, n_a, endpoint=False) + (rs.uniform(0, 0.2) if jitter else 0.0)
+        P.append((e + np.stack([r * np.cos(a), r * np.sin(a)], -1)).reshape(-1, 2))
+    P = np.concatenate(P)
+    return P[(P > 0).all(axis=1) & (P < env.scale).all(axis=1)]
+
+
+def _blocked_big(env, centres, P, want, lo, hi):
+    """Pairs whose straight segment crosses the wall and whose reference rate exceeds 1e-3 of the span."""
+    blocked = O.distances_accounting_for_environment(env, centres, P, "line_of_sight", O.TapeRNG()) == 1000
+    return int((blocked & (np.abs(want - lo) > 1e-3 * abs(hi - lo))).sum())
+
+
 # ---------------------------------------------------------------------------------------------------- PlaceCells
 PC_DESCS = ("gaussian", "gaussian_threshold", "diff_of_gaussians")
 
 
 def _place_case(E, env, Ag, centres, w, geom, P, expect_expanded, tag):
     """Every profile x {uniform, mixed widths} x {min_fr 0 (folded scale), min_fr > 0}: rates against the oracle, and the
-    exponent form the packed meta selects (expanded: one common width, k r2_max <= 10)."""
+    exponent form the packed meta selects (expanded: one common width, k r2_max <= 10, never geodesic).  Geodesic: the
+    sample must hold >= 200 blocked pairs with Gaussian rates above 1e-3 of the span (detours the relative check covers)."""
     rs = np.random.RandomState(11)
     mixed = w * rs.uniform(0.8, 1.25, len(centres))
     for desc in PC_DESCS:
@@ -128,28 +158,38 @@ def _place_case(E, env, Ag, centres, w, geom, P, expect_expanded, tag):
                 c = N._cells()
                 assert (c.k_uniform > 0) == (widths == "uniform")
                 expanded = desc == "gaussian" and c.k_uniform > 0 and c.k_uniform * c.r2_max <= 10 and \
-                    E.boundary_conditions != "periodic"
+                    E.boundary_conditions != "periodic" and geom != "geodesic"
                 assert expanded == (expect_expanded and desc == "gaussian" and widths == "uniform"), (tag, desc, widths)
                 got = N.get_state(evaluate_at=None, pos=P)
                 want = O.place_cells_get_state(env, centres, N.place_cell_widths, P, O.TapeRNG(), desc,
                                                N._effective_geometry(), lo, hi)
                 form = "expanded" if expanded else "direct"
                 _close(got, want, lo, hi, desc == "gaussian", f"{tag} {desc} {widths} widths ({form}) min_fr {lo}")
+                if geom == "geodesic" and desc == "gaussian":
+                    assert N._effective_geometry() == "geodesic"
+                    assert _blocked_big(env, centres, P, want, lo, hi) >= 200, (tag, desc, widths)
                 Ag.Neurons.remove(N)
 
 
-@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight"])
+@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight", "geodesic"])
 @pytest.mark.parametrize("wkind", ["0.2", "0.2*scale", "0.05"])
 @pytest.mark.parametrize("scale", [0.25, 1.0, 2.5, 10.0])
 def test_place_cells_at_scale(scale, wkind, geom):
     w = {"0.2": 0.2, "0.2*scale": 0.2 * scale, "0.05": 0.05}[wkind]
-    E, env = _box(scale, C2 if geom == "line_of_sight" else ())
+    E, env = _box(scale, _walls_of(geom))
     rs = np.random.RandomState(int(scale * 100) + len(wkind))
     centres = _centres(rs, E.extent, 64)
     P = _positions(rs, env, centres, np.full(64, w))
+    expanded = w / scale >= 0.2 - 1e-12
+    if geom == "geodesic":                       # never the expanded form; centres and positions around the wall ends
+        r = min(2.0 * w, 0.25 * scale)
+        near = _around_ends(rs, env, r, n_r=4, n_a=12, jitter=False)
+        centres[4:4 + min(40, len(near))] = near[rs.choice(len(near), min(40, len(near)), replace=False)]
+        P = np.concatenate([P, _around_ends(rs, env, min(3.0 * w, 0.3 * scale))])
+        expanded = False
     Ag = _agent(E)
     # centres inside the box: r2_max = half-diagonal^2, k r2_max = log2(e) (scale / w)^2 / 4, at most 10 for w >= 0.2 scale
-    _place_case(E, env, Ag, centres, w, geom, P, w / scale >= 0.2 - 1e-12, f"scale {scale} w {w} {geom}")
+    _place_case(E, env, Ag, centres, w, geom, P, expanded, f"scale {scale} w {w} {geom}")
 
 
 @pytest.mark.parametrize("w", [0.05, 0.2, 2.0])
@@ -177,15 +217,43 @@ def _edge_positions(rs, centres, r, n_dirs=8):
     return np.concatenate(P)
 
 
-@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight", "periodic"])
+def _detour_edge(rs, env, w, n_c=6, n_dirs=6):
+    """Centres within w of each inner-wall end inside the box, on one side of the wall, and positions on the other side at
+    detour distance |c - e| + |e - p| = w (1 +- eps) for eps in EPS: p = e + (w (1 +- eps) - |c - e|) u, with the centre
+    and u both pointing away from the wall's other end (so the straight segment c -> p crosses the wall)."""
+    C, P = [], []
+    wall = np.asarray(env.walls[4], dtype=float)
+    for k, e in enumerate(wall):
+        if not env.contains(e):
+            continue
+        along = (e - wall[1 - k]) / np.linalg.norm(e - wall[1 - k])      # from the other end out through e
+        side = np.array([-along[1], along[0]])
+        for _ in range(n_c):
+            a = rs.uniform(0.2, 0.8) * w
+            t = rs.uniform(0.15, 0.85) * np.pi / 2                         # back along the wall, on side +1
+            c = e + a * (-np.cos(t) * along + np.sin(t) * side)
+            C.append(c)
+            for eps in EPS:
+                for s in (-1.0, 1.0):
+                    t2 = rs.uniform(0.15, 0.85, n_dirs)[:, None] * np.pi / 2   # back along the wall, on side -1
+                    u = -np.cos(t2) * along - np.sin(t2) * side
+                    P.append(e + (w * (1 + s * eps) - a) * u)
+    return np.array(C), np.concatenate(P)
+
+
+@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight", "periodic", "geodesic"])
 @pytest.mark.parametrize("scale", [1.0, 10.0])
 def test_top_hat_on_the_edge(scale, geom):
     w = 0.1
-    E, env = _box(scale, C2 if geom == "line_of_sight" else (), periodic=geom == "periodic")
+    E, env = _box(scale, _walls_of(geom), periodic=geom == "periodic")
     rs = np.random.RandomState(int(scale) + len(geom))
     centres = _centres(rs, E.extent, 40)
     centres[:4] += np.sign(scale / 2 - centres[:4]) * 1.5 * w          # corner cells with their whole edge in the box
     P = _edge_positions(rs, centres, w)
+    if geom == "geodesic":
+        dc, dp = _detour_edge(rs, env, w)
+        centres = np.concatenate([centres, dc])
+        P = np.concatenate([P, dp])
     if geom == "periodic":
         P = np.mod(P, scale)
     else:
@@ -198,6 +266,11 @@ def test_top_hat_on_the_edge(scale, geom):
                                    scalar_width=w)
     near = np.abs(O.distances_accounting_for_environment(env, centres, P, "euclidean", O.TapeRNG()) / w - 1) < 1e-5
     assert near.sum() > 1000 and 0 < want[near].mean() < 1                  # both sides of the edge are represented
+    if geom == "geodesic":                                                  # and both sides of the detour edge
+        blocked = O.distances_accounting_for_environment(env, centres, P, "line_of_sight", O.TapeRNG()) == 1000
+        dg = O.distances_accounting_for_environment(env, centres, P, "geodesic", O.TapeRNG())
+        edge = blocked & (np.abs(dg / w - 1) < 1e-5)
+        assert edge.sum() > 200 and 0 < want[edge].mean() < 1, edge.sum()
     bad = got != want
     assert not bad.any(), f"{int(bad.sum())} of {bad.size} pairs classified differently (near the edge: {near.sum()})"
 
@@ -256,11 +329,12 @@ def _one_hot_layout(scale, periodic):
     return np.concatenate(C), (np.mod(P, scale) if periodic else P)
 
 
-@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight", "periodic"])
+@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight", "periodic", "geodesic"])
 @pytest.mark.parametrize("scale", [1.0, 10.0])
 def test_one_hot_arg_min_at_scale(scale, geom):
     periodic = geom == "periodic"
-    walls = C2 + [[[0.9, 0.85], [0.9, 0.95]]] if geom == "line_of_sight" else ()   # the last wall cuts through the grid
+    cut = [[[0.9, 0.85], [0.9, 0.95]]]                                       # a wall through the grid
+    walls = {"line_of_sight": C2 + cut, "geodesic": cut}.get(geom, ())
     E, env = _box(scale, walls, periodic=periodic)
     centres, P = _one_hot_layout(scale, periodic)
     Ag = _agent(E)
@@ -382,35 +456,42 @@ def test_vector_cells_at_scale_10():
         _close(A.get_state(evaluate_at=None, pos=X, other_pos=Y), want, 0, 1, False, f"avc occlude {occlude}")
 
 
-@pytest.mark.parametrize("geom", ["euclidean", "line_of_sight"])
-def test_phase_precessing_place_cells_at_scale_10(geom):
-    E, env = _box(10.0, C2 if geom == "line_of_sight" else ())
+@pytest.mark.parametrize("geom,w", [("euclidean", 0.2), ("line_of_sight", 0.2), ("geodesic", 0.2), ("geodesic", 0.05)])
+def test_phase_precessing_place_cells_at_scale_10(geom, w):
+    E, env = _box(10.0, _walls_of(geom))
     rs = np.random.RandomState(6)
     centres = _centres(rs, E.extent, 40)
-    P = _positions(rs, env, centres, np.full(40, 0.2), n_random=600, n_ring_centres=8)
-    _pppc_at(E, env, centres, 0.2, P, f"pppc scale 10 {geom}", geom)
+    P = _positions(rs, env, centres, np.full(40, w), n_random=600, n_ring_centres=8)
+    if geom == "geodesic":
+        near = _around_ends(rs, env, 2.0 * w, n_r=4, n_a=6, jitter=False)
+        n = min(36, len(near))
+        centres[4:4 + n] = near[:n]
+        P = np.concatenate([P, _around_ends(rs, env, 3.0 * w, n_r=8, n_a=12)])
+    _pppc_at(E, env, centres, w, P, f"pppc scale 10 {geom} w {w}", geom)
 
 
 def test_random_spatial_neurons_large_box():
     """The sample grid has 0.05 m spacing whatever the lengthscale, so a scale-10 box would need a 40 000^2 covariance at
     set-up: the box is 2.5 m with a 5 cm lengthscale instead (L / w = 50, as scale 10 with w = 0.2)."""
-    E, env = _box(2.5, C2)
     rs = np.random.RandomState(8)
     np.random.seed(8)
-    Ag = _agent(E)
-    for geom in ("euclidean", "line_of_sight"):
+    for geom in ("euclidean", "line_of_sight", "geodesic"):
+        E, env = _box(2.5, GEO if geom == "geodesic" else C2)
+        Ag = _agent(E)
         N = rb.RandomSpatialNeurons(Ag, {"n": 12, "lengthscale": 0.05, "wall_geometry": geom})
+        assert N._effective_geometry() == geom
         P = _positions(rs, env, N.X, np.full(len(N.X), 0.05), n_random=1000, n_ring_centres=8)
         want = R.get_state(env, N.X, N.targets, N.lengthscale, geom, P, O.TapeRNG())
         _close(N.get_state(evaluate_at=None, pos=P), want, 0, 1, False, f"rsn {geom}")
 
 
 # ----------------------------------------------------------------------------------------- launch paths at scale 10
-@pytest.mark.parametrize("kind,w", [("place_los", 0.2), ("place_los", 0.05), ("place", 0.2), ("place", 0.05), ("grid", None)])
+@pytest.mark.parametrize("kind,w", [("place_los", 0.2), ("place_los", 0.05), ("place", 0.2), ("place", 0.05),
+                                    ("place_geo", 0.2), ("place_geo", 0.05), ("grid", None)])
 def test_run_and_stepped_updates_at_scale_10(kind, w):
     """The agent records are built by the step kernel's producer warps on these paths (not by get_state): the whole-run
     launch of one population, then the stepped API, against the oracle at Ag.pos."""
-    E, env = _box(10.0, C2 if kind == "place_los" else ())
+    E, env = _box(10.0, {"place_los": C2, "place_geo": GEO_END}.get(kind, ()))
     np.random.seed(2)
     A = 700
     Ag = rb.Agent(E, {"dt": 0.05, "n_agents": A, "seed": 5, "speed_mean": 0.5})
@@ -418,8 +499,9 @@ def test_run_and_stepped_updates_at_scale_10(kind, w):
         N = rb.GridCells(Ag, {"n": 48})
         oracle = lambda pos: O.grid_cells_get_state(N.gridscales, N.phase_offsets, N.w, pos).T
     else:
-        geom = "line_of_sight" if kind == "place_los" else "euclidean"
+        geom = {"place_los": "line_of_sight", "place_geo": "geodesic"}.get(kind, "euclidean")
         N = rb.PlaceCells(Ag, {"n": 200, "widths": w, "wall_geometry": geom})
+        assert N._effective_geometry() == geom
         assert not (N._cells().k_uniform * N._cells().r2_max <= 10)             # the direct exponent form
         oracle = lambda pos: O.place_cells_get_state(env, N.place_cell_centres, N.place_cell_widths, pos, O.TapeRNG(),
                                                      "gaussian", geom).T
