@@ -325,41 +325,53 @@ __device__ __forceinline__ void spike_store(const uint32_t (&b)[4], uint32_t* sp
       "@p st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};\n\t}" ::"l"(spk), "r"(b[0]), "r"(b[1]), "r"(b[2]), "r"(b[3])
       : "memory");
 }
-// one agent (whole warp must call)
-__device__ __forceinline__ void spikes1(const float (&o)[4], const OutK& out, const TailCtx& t, const RowCursor& rc) {
-  uint32_t c[4], b[4];
-  spike_words(c, out, t, rc.gid);
-  const float nv = spike_neg_dither(c);
-  const unsigned h = (unsigned)(rc.gid & 1ull);
-  spike_ballots<true>(b, h ? c[2] : c[0], h ? c[3] : c[1], nv, o, out.dt * 65536.0f, t.vmask, true);
-  spike_store(b, rc.spk);
+// A position in a ring slot's spike staging block (shared memory, same layout as the global rows; see k_step): the whole
+// run's consumers store their ballot words there, and the slot's producer writes the block to HBM as whole lines.
+struct SmemSpk { uint32_t addr; };
+__device__ __forceinline__ SmemSpk operator+(const SmemSpk p, const long long words) { return {p.addr + 4u * (uint32_t)words}; }
+__device__ __forceinline__ SmemSpk& operator+=(SmemSpk& p, const long long words) { p.addr += 4u * (uint32_t)words; return p; }
+__device__ __forceinline__ void spike_store(const uint32_t (&b)[4], const SmemSpk spk) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "elect.sync _|p, 0xffffffff;\n\t"
+      "@p st.shared.v4.u32 [%0], {%1,%2,%3,%4};\n\t}" ::"r"(spk.addr), "r"(b[0]), "r"(b[1]), "r"(b[2]), "r"(b[3])
+      : "memory");
 }
-// agents rc.gid and, if has_b, rc.gid + 1 of the general path (whole warp must call): one Philox call for a complete pair
+// one agent (whole warp must call); SP: uint32_t* (global row) or SmemSpk (staging block)
+template <class SP>
+__device__ __forceinline__ void spikes1(const float (&o)[4], const OutK& out, const TailCtx& t, const unsigned long long gid,
+                                        const SP spk) {
+  uint32_t c[4], b[4];
+  spike_words(c, out, t, gid);
+  const float nv = spike_neg_dither(c);
+  const unsigned h = (unsigned)(gid & 1ull);
+  spike_ballots<true>(b, h ? c[2] : c[0], h ? c[3] : c[1], nv, o, out.dt * 65536.0f, t.vmask, true);
+  spike_store(b, spk);
+}
+// agents gid and, if has_b, gid + 1 of the general path (whole warp must call): one Philox call for a complete pair
 // that starts on an even id, else one per agent
+template <class SP>
 __device__ __forceinline__ void spikes_pair(const float (&oa)[4], const float (&ob)[4], const bool has_b, const bool even,
-                                            const OutK& out, const TailCtx& t, const RowCursor& rc, const float q16) {
+                                            const OutK& out, const TailCtx& t, const unsigned long long gid, const SP spk,
+                                            const float q16) {
   if (has_b && even) {
     uint32_t c[4], bl[4];
-    spike_words(c, out, t, rc.gid);
+    spike_words(c, out, t, gid);
     const float nv = spike_neg_dither(c);
     spike_ballots<true>(bl, c[0], c[1], nv, oa, q16, t.vmask, true);
-    spike_store(bl, rc.spk);
+    spike_store(bl, spk);
     spike_ballots<true>(bl, c[2], c[3], nv, ob, q16, t.vmask, true);
-    spike_store(bl, rc.spk + out.spike_ld);
+    spike_store(bl, spk + out.spike_ld);
   } else {
-    spikes1(oa, out, t, rc);
-    if (has_b) {
-      RowCursor rb = rc;
-      rb.gid += 1; rb.spk += out.spike_ld;
-      spikes1(ob, out, t, rb);
-    }
+    spikes1(oa, out, t, gid, spk);
+    if (has_b) spikes1(ob, out, t, gid + 1ull, spk + out.spike_ld);
   }
 }
 
 template <bool SPIKES, bool NOISE>
 __device__ __forceinline__ void finish4(float (&o)[4], const OutK& out, const TailCtx& t, const RowCursor& rc) {
   store4<NOISE>(o, out, t, rc, 0);
-  if (SPIKES && (!NOISE || rc.spk != nullptr)) spikes1(o, out, t, rc);
+  if (SPIKES && (!NOISE || rc.spk != nullptr)) spikes1(o, out, t, rc.gid, rc.spk);
 }
 
 // ---------------------------------------------------------------------------
@@ -655,7 +667,7 @@ struct __align__(16) StepSlot {
   float rec[TA][REC];
   int na;
   unsigned nanmask;         // bit a: agent a's position is NaN -> its rates are zero (Neurons.py:163-164)
-  int pad[2];
+  uint32_t* spk_rows;       // whole run, dense spikes: the tile's first spike row, where its staging block goes (k_step)
 };
 
 // The consumers' hot loop: n2 consecutive agent pairs (2p, 2p+1) of one ring slot, no OU noise, 16-byte aligned rows
@@ -665,10 +677,10 @@ struct __align__(16) StepSlot {
 // those pairs through the general path (per-agent exact float64 fall-back) after the loop -- no call, no branch in here.
 // DENSE: the dense spike stream (one Philox4x32-7 call per pair, a threshold test per rate; needs an even first global
 // id) runs in the loop; thinned spikes are a post-pass over the slot (thin_block) and leave this loop spike-free.
-template <class P, bool DENSE, int EXP>
+template <class P, bool DENSE, int EXP, class SP>
 __device__ __forceinline__ void consume_pairs(const int n2, const typename P::Regs& regs, const typename P::Const& pc,
                                               const OutK& out, const TailCtx& tc, const int cell0, const float*& recp,
-                                              const uint32_t inner_s, const long long ld, float*& d, uint32_t*& spk,
+                                              const uint32_t inner_s, const long long ld, float*& d, SP& spk,
                                               unsigned long long& pair, const bool act, const float q16, uint32_t& redo) {
   for (int it = 0; it < n2; ++it) {
     float o[4];
@@ -874,7 +886,7 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
           }
           store4<NOISE>(oa, out, tc, rc, 0);
           if (has_b) store4<NOISE>(ob, out, tc, rc, out.ld);
-          if (DENSE && (!NOISE || rc.spk != nullptr)) spikes_pair(oa, ob, has_b, even, out, tc, rc, q16);
+          if (DENSE && (!NOISE || rc.spk != nullptr)) spikes_pair(oa, ob, has_b, even, out, tc, rc.gid, rc.spk, q16);
           cursor_advance(rc, stride);
           recp += 2 * P::REC;
         }
@@ -891,11 +903,12 @@ __device__ __forceinline__ void consumer_slots(const typename P::Const& pc, cons
 
 // Repairs of one ring slot for consumer_fast, after its pair loop (rare): pairs whose float32 line-of-sight decision fell
 // inside the band (bit `it` of redo) are re-evaluated with the exact float64 fall-back, and an odd last agent gets its row.
-// Inlined like the pair loop; only the float64 fall-back (place_blocked_exact4) is an out-of-line call.
-template <class P, bool DENSE>
+// Inlined like the pair loop; only the float64 fall-back (place_blocked_exact4) is an out-of-line call.  spk: this warp's
+// ballot words in the tile's first spike row (global, or the slot's staging block: the pair loop's words are overwritten there).
+template <class P, bool DENSE, class SP>
 __device__ __forceinline__ void slot_fixups(const typename P::Regs& regs, const typename P::Const& pc, const OutK& out,
                                             const TailCtx& tc, const float* rec, const uint32_t inner_s, float* d,
-                                            uint32_t* spikes, const long long a0, const int n_agents, const uint32_t redo,
+                                            const SP spk, const long long a0, const int n_agents, const uint32_t redo,
                                             const bool act) {
   for (int a = 0; a < n_agents; a += 2, d += 2 * out.ld, rec += 2 * P::REC) {
     const bool has_b = a + 1 < n_agents;
@@ -908,23 +921,22 @@ __device__ __forceinline__ void slot_fixups(const typename P::Regs& regs, const 
       st_cs_f4(d, oa);
       if (has_b) st_cs_f4(d + out.ld, ob);
     }
-    if constexpr (DENSE) {                                          // whole warp: ballots
-      RowCursor rc;
-      rc.gid = (unsigned long long)(out.id_offset + a0 + a);
-      rc.spk = spikes + (a0 + a) * out.spike_ld + ((tc.cell0 >> 7) << 2);
-      spikes_pair(oa, ob, has_b, true, out, tc, rc, out.dt * 65536.0f);   // even: consumer_fast's tiles start on even ids
-    }
+    if constexpr (DENSE)                                            // whole warp: ballots; even: consumer_fast's tiles start on even ids
+      spikes_pair(oa, ob, has_b, true, out, tc, (unsigned long long)(out.id_offset + a0 + a), spk + a * out.spike_ld, out.dt * 65536.0f);
   }
 }
 
 // The consumers' slot loop for the common case: no OU noise, vector-aligned rows, whole 4-cell groups, all cells resident
 // in one set of registers (n_pad <= 2048), an even first global id when there are spikes.  Pointers advance incrementally,
-// the rare repairs run after the pair loop (slot_fixups), thinned spikes are a post-pass per slot (thin_block).
+// the rare repairs run after the pair loop (slot_fixups), thinned spikes are a post-pass per slot (thin_block).  The whole
+// run's dense spike words go to the slot's staging block at `stage` (shared address, see k_step), the stepped paths' to HBM.
 template <class P, int SPK, class C, int EXP, bool MULTI>
 __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const OutK& out, const RunK& run, StepSlot<P::REC>* s_slot,
                                               uint64_t* s_full, uint64_t* s_empty, const double* s_walls, const long long nq,
-                                              const int ctid, const int lane, const long long n_rows) {
+                                              const int ctid, const int lane, const long long n_rows, const uint32_t stage) {
   constexpr int NS = ring_slots<P, C>(), MW = C::MW, NSP = NS / MW;
+  constexpr bool STAGED = MULTI && SPK == 1;
+  using SP = std::conditional_t<STAGED, SmemSpk, uint32_t*>;
   const int CT = pc.n_pad / 4;                        // cell-threads needed (multiple of 32, <= RW * 32)
   const int G = lean_groups(CT, NS), grp = ctid / CT; // groups of CT threads; group g consumes the tiles q = g, g + G, ...
   if (grp >= G) return;                               // spare warps (the slots' release count is one group's warps)
@@ -966,10 +978,15 @@ __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const
         float* d = dst0;
         uint32_t redo = 0u;
         const int n2 = (a_hi - a_lo) >> 1;
-        uint32_t* spk = nullptr;
+        const auto first_spk = [&]() -> SP {                             // this warp's words in the tile's first spike row
+          if constexpr (STAGED) return SmemSpk{stage + 4u * (uint32_t)(s * TA * out.spike_ld + ((cell0 >> 7) << 2))};
+          else if constexpr (SPK == 1) return spikes + a0 * out.spike_ld + ((cell0 >> 7) << 2);
+          else return nullptr;
+        };
+        SP spk{};
         unsigned long long pair = 0ull;
         if constexpr (SPK == 1) {
-          spk = spikes + a0 * out.spike_ld + ((cell0 >> 7) << 2);
+          spk = first_spk();
           pair = (unsigned long long)(out.id_offset + a0) >> 1;          // even first global id: rows (2p, 2p+1) are one pair
         }
         consume_pairs<P, SPK == 1, EXP>(n2, regs, pc, out, tc, cell0, recp, inner_s, ld, d, spk, pair, act, q16, redo);
@@ -979,7 +996,7 @@ __device__ __forceinline__ void consumer_fast(const typename P::Const& pc, const
           // schedules 65 of the k_step instantiations differently; they stay until a measurement says which is faster
           const typename P::Regs rcopy = regs;
           const typename P::Const pcopy = pc;
-          slot_fixups<P, SPK == 1>(rcopy, pcopy, out, tc, s_slot[s].rec[a_lo], inner_s, dst0, spikes, a0, a_hi - a_lo, redo, act);
+          slot_fixups<P, SPK == 1>(rcopy, pcopy, out, tc, s_slot[s].rec[a_lo], inner_s, dst0, first_spk(), a0, a_hi - a_lo, redo, act);
         }
         if (const unsigned nm = s_slot[s].nanmask; nm != 0u && act) {     // NaN position -> zero rates (Neurons.py:163-164)
           for (int a = a_lo; a < a_hi; ++a)
@@ -1013,6 +1030,21 @@ __device__ __forceinline__ void clear_spike_row(uint32_t* row, const long long w
     asm volatile("st.global.cs.v4.u32 [%0], {%1,%1,%1,%1};" ::"l"(row + w), "r"(0u) : "memory");
 }
 
+// Whole run with the dense stream: a producer writes the staging block of a consumed tile (`words` words from shared address
+// `src`) to its spike rows at `dst`.  Rows of consecutive agents are contiguous, so the block is one range of whole lines:
+// 512 B per warp instruction, instead of the 16-byte pieces each consumer warp would store into every row.
+__device__ __forceinline__ void flush_spike_block(uint32_t* dst, const uint32_t src, const int words, const int lane) {
+#pragma unroll 4
+  for (int w = 4 * lane; w < words; w += 128) {
+    uint32_t v0, v1, v2, v3;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3) : "r"(src + 4u * (uint32_t)w) : "memory");
+    asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(dst + w), "r"(v0), "r"(v1), "r"(v2), "r"(v3) : "memory");
+  }
+}
+
+// bytes of dynamic shared memory k_step needs: the whole run's dense spike staging, one block of TA rows per ring slot
+__host__ __device__ constexpr long long spike_stage_bytes(int ring, long long spike_ld) { return (long long)ring * TA * spike_ld * 4; }
+
 // SPK: 0 no spikes, 1 dense spike stream (in the loops), 2 thinned spikes (thin_block per ring slot)
 template <class P, int MODE, int SPK, bool NOISE, class C>
 __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, const riab_agents ag,
@@ -1024,6 +1056,11 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
   constexpr int MW = C::MW, NS = ring_slots<P, C>();
   __shared__ StepSlot<P::REC> s_slot[NS];
   __shared__ uint64_t s_bar, s_full[NS], s_empty[NS];
+  // whole run, dense spikes: slot s's spike words are assembled in s_stage[s * TA * spike_ld ..] (rows of the tile, laid out
+  // like the global rows) and written to HBM by the slot's producer once the consumers have released the slot
+  constexpr bool STAGED = MODE >= 3 && SPK == 1 && !NOISE;
+  extern __shared__ __align__(128) unsigned char dyn[];
+  const uint32_t s_stage = smem_u32(dyn);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // lean consumers (consumer_fast): every ring slot is consumed by ONE group of warps (n_pad / 4 threads), the general
   // loop (consumer_slots) by all RW consumer warps
@@ -1068,9 +1105,13 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
         for (long long q = pw; q < nq; q += MW, ++n) {
           const int s = pw + MW * (int)(n % NSP);
           mbar_wait(&s_empty[s], (uint32_t)(((n / NSP) & 1) ^ 1));
+          // the wait acquired the consumers' staging stores of the tile this slot held (record n - NSP): write them out
+          if constexpr (STAGED)
+            if (n >= NSP) flush_spike_block(s_slot[s].spk_rows, s_stage + (uint32_t)spike_stage_bytes(s, out.spike_ld), s_slot[s].na * (int)out.spike_ld, lane);
           const long long a0 = ((long long)blockIdx.x + q * gridDim.x) * ta;
           const int na = (int)((n_rows - a0) < ta ? (n_rows - a0) : ta);
           if (SPK == 2 && lane < na && spikes_st != nullptr) clear_spike_row(spikes_st + (a0 + lane) * out.spike_ld, out.spike_ld);
+          if (STAGED && lane == 0) s_slot[s].spk_rows = spikes_st + a0 * out.spike_ld;     // (publish_slot's __syncwarp orders it)
           bool nanpos = false;
           if (lane < na) {
             AgentState as;
@@ -1082,6 +1123,15 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
           publish_slot(s_slot[s], &s_full[s], lane, na, nanpos);
         }
         if constexpr (MODE == 4) t_st = t_st + mp.dt;
+      }
+      if constexpr (STAGED) {
+        // the blocks of this warp's last NSP records i: their consumers complete phase i / NSP of s_empty, the phase a
+        // refill (record i + NSP) would wait for with parity ((i + NSP) / NSP & 1) ^ 1 = (i / NSP) & 1
+        for (long long i = (n > NSP ? n - NSP : 0); i < n; ++i) {
+          const int s = pw + MW * (int)(i % NSP);
+          mbar_wait(&s_empty[s], (uint32_t)((i / NSP) & 1));
+          flush_spike_block(s_slot[s].spk_rows, s_stage + (uint32_t)spike_stage_bytes(s, out.spike_ld), s_slot[s].na * (int)out.spike_ld, lane);
+        }
       }
     } else {
       for (long long q = pw; q < nq; q += MW) {
@@ -1139,9 +1189,9 @@ __global__ void __launch_bounds__(C::THREADS, C::CTAS) k_step(const EnvK env, co
     const int ex = P::expanded(pc);
     if constexpr (!NOISE) {
       if (lean) {
-        if (ex == 2) consumer_fast<P, SPK, C, 2, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
-        else if (ex == 1) consumer_fast<P, SPK, C, 1, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
-        else consumer_fast<P, SPK, C, 0, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows);
+        if (ex == 2) consumer_fast<P, SPK, C, 2, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows, s_stage);
+        else if (ex == 1) consumer_fast<P, SPK, C, 1, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows, s_stage);
+        else consumer_fast<P, SPK, C, 0, (MODE >= 3)>(pc, out, run, s_slot, s_full, s_empty, s_walls, nq, ctid, lane, n_rows, s_stage);
         return;
       }
     }
@@ -1952,8 +2002,18 @@ int launch_tile(const EnvK& env, const riab_agents& ag, const riab_motion_params
   else if (spikes) {
     // dense stream: light consumers (Euclidean Gaussian place cells) are producer-bound next to 4 producer warps and get 8;
     // the heavier loops keep the 104-register consumers
-    if constexpr (P::LIGHT) k_step<P, MODE, 1, false, StepCfg<12>><<<grid, StepCfg<12>::THREADS, 0, s>>>(env, ag, mp, md, io, pc, out, pos_in, n_rows, run);
-    else k_step<P, MODE, 1, false, StepCfg<4>><<<grid, StepCfg<4>::THREADS, 0, s>>>(env, ag, mp, md, io, pc, out, pos_in, n_rows, run);
+    using C = std::conditional_t<P::LIGHT, StepCfg<12>, StepCfg<4>>;
+    auto* kern = k_step<P, MODE, 1, false, C>;
+    size_t stage = 0;
+    if (MODE >= 3) {
+      // the whole run assembles the spike rows in shared memory (k_step): the opt-in covers the largest population the
+      // lean loop takes (RW * 32 * 4 cells); the attribute belongs to the current device's function image, so it is set
+      // per launch (a single process may drive several GPUs)
+      RIAB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)spike_stage_bytes(ring_slots<P, C>(), RW * 32 * 4 / 32)));
+      stage = (size_t)spike_stage_bytes(ring_slots<P, C>(), out.spike_ld);
+    }
+    kern<<<grid, C::THREADS, stage, s>>>(env, ag, mp, md, io, pc, out, pos_in, n_rows, run);
   }
   else {
     // light consumers without spikes run at the HBM write rate: fat producers (only instantiated for them)
