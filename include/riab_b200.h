@@ -55,7 +55,16 @@ typedef enum { RIAB_BOUNDARY_SOLID_BOX = 0, RIAB_BOUNDARY_PERIODIC_BOX = 1, RIAB
 /* ---------------------------------------------------------------- Environment
  * walls: (n_walls,2,2) float64, boundary walls first (Environment.py:137-144),
  * then user walls (add_wall, :330-342), then the walls of the holes (:147-160).  2D: rectangular box (solid or
- * periodic), or a polygon boundary and / or holes (solid). */
+ * periodic), or a polygon boundary and / or holes (solid).
+ *
+ * Wall count: every entry point accepts up to RIAB_MAX_WALLS walls for what reads no walls or reads them in the motion
+ * and BVC ray kernels (the stepped motion, SubAgents, ThetaSequenceAgent, BVCs, and the populations below that ignore
+ * walls).  Rates that read walls keep RIAB_MAX_STEP_WALLS: line_of_sight / geodesic PlaceCells, PhasePrecessingPlaceCells
+ * and RandomSpatialNeurons (and so the SpatialGoalEnvironment goal test), ObjectVectorCells / AgentVectorCells with
+ * walls_occlude.  Above RIAB_MAX_STEP_WALLS, riab_step_fused and riab_run run the stand-alone motion kernel and then
+ * each population (no fused, skewed or whole-run launch). */
+#define RIAB_MAX_WALLS 1024
+#define RIAB_MAX_STEP_WALLS 64        /* walls the rate kernels (k_step, k_place_onehot, k_rsn) stage */
 typedef struct {
   const double* walls_dev;     /* device, n_walls*4 doubles */
   int32_t n_walls;
@@ -126,7 +135,7 @@ typedef struct {
 #define RIAB_MAX_REC_ITERS 4
 #define RIAB_MAX_BOUNCE_ITERS 32
 
-/* Agent.update (Agent.py:160-242, random-motion branch) for n_agents agents. */
+/* Agent.update (Agent.py:160-242, random-motion branch) for n_agents agents; up to RIAB_MAX_WALLS walls. */
 int riab_agent_update(const riab_agents* agents, const riab_env* env,
                       const riab_motion_params* prm, const riab_step_io* io, void* stream);
 
@@ -447,6 +456,7 @@ typedef struct {
   float* bvc_scratch;      /* (A, T) f32, BVC only */
 } riab_rates_out;
 
+/* Above RIAB_MAX_STEP_WALLS walls the motion kernel runs first, then the population's rate kernel. */
 int riab_step_fused(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm,
                     const riab_step_io* io, int32_t cells_kind, const void* cells /* riab_place_cells* etc. */,
                     const riab_neuron_noise* noise, const riab_rates_out* out, void* stream);
@@ -730,6 +740,7 @@ typedef struct {
   int32_t ring_next;
 } riab_agent_history;
 
+/* Above RIAB_MAX_STEP_WALLS walls every step is the motion kernel, then each population (no whole-run or skewed launch). */
 int riab_run(const riab_agents* agents, const riab_env* env, const riab_motion_params* prm, const riab_step_io* io,
              const riab_population* pops, int32_t n_pops, const riab_agent_history* hist, int64_t n_steps,
              void* stream);

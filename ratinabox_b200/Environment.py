@@ -143,9 +143,10 @@ class Environment:
             positions[:, 0] = np.random.uniform(ex[0], ex[1], size=n)
             positions[:, 1] = np.random.uniform(ex[2], ex[3], size=n)
             if self.is_polygonal:                                   # :592-600 brute-force resampling
-                for i, pos in enumerate(positions):
-                    if self.check_if_position_is_in_environment(pos) == False:
-                        positions[i] = self.sample_positions(n=1, method="random").reshape(-1)
+                # one vectorised test of the n draws, then the reference's draw order: each outside point, in index
+                # order, re-drawn by its own sample_positions(n=1) call
+                for i in np.flatnonzero(~self._in_environment(positions)):
+                    positions[i] = self.sample_positions(n=1, method="random").reshape(-1)
             return positions
         if method[:7] == "uniform":
             area = (ex[1] - ex[0]) * (ex[3] - ex[2])
@@ -156,8 +157,7 @@ class Environment:
             y = np.linspace(ex[2] + delta / 2, ex[3] - delta / 2, int((ex[3] - ex[2]) / delta))
             positions = np.array(np.meshgrid(x, y)).reshape(2, -1).T
             if self.is_polygonal:                                   # :612-615 drop the illegal grid points
-                delpos = [i for (i, pos) in enumerate(positions) if self.check_if_position_is_in_environment(pos) == False]
-                positions = np.delete(positions, delpos, axis=0)
+                positions = positions[self._in_environment(positions)]
             n_uniform = positions.shape[0]
             if method[7:] == "_jitter":
                 positions = positions + np.random.uniform(-0.45 * delta, 0.45 * delta, positions.shape)
@@ -188,6 +188,17 @@ class Environment:
             is_in = is_in and not _polygon_contains_strict(h, pos)
         return bool(is_in)
 
+    def _in_environment(self, positions):
+        """check_if_position_is_in_environment of every row of an (m, 2) array of a polygonal environment, as a bool
+        array: the same float64 decisions as the scalar test (which a few points take: it is faster there, and
+        sample_positions re-draws outside points one at a time)."""
+        if len(positions) <= 4:
+            return np.array([self.check_if_position_is_in_environment(p) for p in positions], dtype=bool)
+        is_in = _polygon_contains_strict_many(self.boundary, positions)
+        for h in self.holes:
+            is_in &= ~_polygon_contains_strict_many(h, positions)
+        return is_in
+
 
 def _polygon_contains_strict(verts, p):
     """Even-odd ray cast; points on an edge or a vertex are NOT inside (shapely ``contains``,
@@ -206,6 +217,26 @@ def _polygon_contains_strict(verts, p):
             if x < xi:
                 inside = not inside
     return inside
+
+
+def _polygon_contains_strict_many(verts, points):
+    """_polygon_contains_strict of every row of an (m, 2) array: the same float64 operations in the same order, one
+    edge at a time over all points, so every decision equals the scalar one."""
+    pts = np.asarray(points, dtype=float).reshape(-1, 2)
+    x, y = pts[:, 0], pts[:, 1]
+    n = len(verts)
+    inside = np.zeros(len(pts), dtype=bool)
+    on_edge = np.zeros(len(pts), dtype=bool)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        for i in range(n):
+            x0, y0 = float(verts[i][0]), float(verts[i][1])
+            x1, y1 = float(verts[(i + 1) % n][0]), float(verts[(i + 1) % n][1])
+            cross = (x1 - x0) * (y - y0) - (y1 - y0) * (x - x0)
+            on_edge |= (cross == 0.0) & (min(x0, x1) <= x) & (x <= max(x0, x1)) & (min(y0, y1) <= y) & (y <= max(y0, y1))
+            straddles = (y0 > y) != (y1 > y)                 # implies y1 != y0: the division below is only used there
+            xi = x0 + (y - y0) * (x1 - x0) / (y1 - y0)
+            inside ^= straddles & (x < xi)
+    return inside & ~on_edge
 
 
 def _polygon_area(verts):

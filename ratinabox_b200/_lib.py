@@ -218,6 +218,8 @@ KIN_HEAD_DIRECTION, KIN_VELOCITY, KIN_SPEED = 0, 1, 2                # riab_kin_
 PLACE_MAX_WI = 8                                              # inner walls of the line-of-sight / geodesic kernels
 ACTIVATIONS = {"linear": 0, "sigmoid": 1, "relu": 2, "tanh": 3, "retanh": 4, "softmax": 5}   # riab_activation
 MAX_REC_ITERS = 4
+MAX_WALLS = 1024                                              # RIAB_MAX_WALLS: walls of the motion and BVC kernels
+MAX_STEP_WALLS = 64                                           # RIAB_MAX_STEP_WALLS: walls of the rate kernels that read them
 
 # name -> (restype, argtypes); every symbol include/riab_b200.h declares
 SYMBOLS = {

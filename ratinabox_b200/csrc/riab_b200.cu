@@ -65,7 +65,10 @@ int fail(int code, const char* fmt, ...) {
 
 constexpr int TA = 32;      // agents per tile (one warp runs their motion)
 constexpr int NT = 256;     // threads per CTA in the tile kernels
-constexpr int MAXW = 64;    // walls staged in shared memory
+constexpr int MAXW = RIAB_MAX_STEP_WALLS;    // walls the rate kernels stage in static shared memory
+// The motion kernels (k_agent_update, k_subagent, k_theta_seq) stage all RIAB_MAX_WALLS walls in dynamic shared memory,
+// W * 32 bytes: within the 48 KB every kernel may use without an opt-in.
+static_assert(RIAB_MAX_WALLS * 32 <= 48 * 1024, "motion wall staging needs no dynamic shared memory opt-in");
 constexpr int CELL_PAD = 128;  // packed per-cell arrays are padded to 4 cells x 32 lanes
 
 struct EnvK {
@@ -177,10 +180,12 @@ __global__ void __launch_bounds__(128) k_agent_update_src(const riab_agents ag, 
   agent_update_src_one(ag, mp, md, io, src, src.t, env, i, s);
 }
 
+// dynamic shared memory: env.W * 32 bytes of walls (motion_walls_bytes)
 template <bool REC>
 __global__ void __launch_bounds__(128) k_agent_update(const riab_agents ag, const riab_motion_params mp,
                                                       const MotionDerived md, const riab_step_io io, const EnvK env) {
-  __shared__ __align__(16) double s_walls[MAXW * 4];
+  extern __shared__ __align__(128) unsigned char dyn[];
+  double* s_walls = reinterpret_cast<double*>(dyn);
   __shared__ uint64_t s_bar;
   stage_walls(s_walls, &s_bar, env);
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1320,7 +1325,9 @@ __global__ void __launch_bounds__(NT) k_finish_rows(const OutK out, const int n_
 }
 
 // ---------------------------------------------------------------------------
-// BVC phase A: one CTA per tile of 32 agents.
+// BVC phase A: one CTA per tile of 32 agents.  Dynamic shared memory: the T directions, then (TABLE) the float32
+// directions and the (angle, wall) table of at most BVC_NW walls next to the static wall block, or (!TABLE) the env.W
+// float64 walls and their float32 copies (launch_bvc), up to RIAB_MAX_WALLS.
 template <bool TABLE>
 __global__ void __launch_bounds__(NT, TABLE ? 4 : 1) k_bvc_rays(const EnvK env, const BvcConst bc,
                                                  const double* __restrict__ pos_in, const long long n_rows,
@@ -1328,8 +1335,10 @@ __global__ void __launch_bounds__(NT, TABLE ? 4 : 1) k_bvc_rays(const EnvK env, 
                                                  uint32_t* __restrict__ spikes_zero, const long long spike_ld) {
   extern __shared__ __align__(128) unsigned char dyn[];
   double* s_dirs = reinterpret_cast<double*>(dyn);                 // T*2
-  __shared__ __align__(16) double s_walls[MAXW * 4];
-  __shared__ __align__(16) float4 s_wf[MAXW];
+  __shared__ __align__(16) double s_walls_tab[TABLE ? MAXW * 4 : 2];
+  __shared__ __align__(16) float4 s_wf_tab[TABLE ? MAXW : 1];
+  double* s_walls = TABLE ? s_walls_tab : s_dirs + 2 * bc.T;         // 16-byte aligned: T * 16 bytes of directions
+  float4* s_wf = TABLE ? s_wf_tab : reinterpret_cast<float4*>(s_walls + 4 * env.W);
   __shared__ __align__(16) double s_pos[TA][2];
   __shared__ uint64_t s_bar;
   stage_walls(s_walls, &s_bar, env);
@@ -1651,7 +1660,8 @@ __global__ void __launch_bounds__(NT) k_history_maps(const riab_history_view h, 
 // host helpers
 int make_env(const riab_env* env, EnvK& k) {
   if (env == nullptr || (env->walls_dev == nullptr && env->n_walls > 0)) return fail(RIAB_ERR_INVALID, "env / walls_dev is NULL");
-  if (env->n_walls < 0 || env->n_walls > MAXW) return fail(RIAB_ERR_UNSUPPORTED, "n_walls=%d exceeds %d", env->n_walls, MAXW);
+  if (env->n_walls < 0 || env->n_walls > RIAB_MAX_WALLS)
+    return fail(RIAB_ERR_UNSUPPORTED, "n_walls=%d exceeds %d", env->n_walls, RIAB_MAX_WALLS);
   if (env->n_boundary_walls < 0 || env->n_boundary_walls > env->n_walls)
     return fail(RIAB_ERR_INVALID, "n_boundary_walls=%d out of range", env->n_boundary_walls);
   k.walls = env->walls_dev; k.W = env->n_walls; k.nb = env->n_boundary_walls;
@@ -1670,6 +1680,21 @@ int make_env(const riab_env* env, EnvK& k) {
   k.scale = env->scale;
   if (k.periodic && !(env->scale > 0.0)) return fail(RIAB_ERR_INVALID, "periodic environment needs scale > 0");
   return 0;
+}
+
+// Dynamic shared memory of the motion kernels: every wall in float64
+size_t motion_walls_bytes(const EnvK& env) { return (size_t)env.W * 4 * sizeof(double); }
+
+// Whether the motion step can run inside a rate kernel (k_step MODE 1 / 2 / 3 / 4), whose static wall block holds MAXW
+// walls; with more, the stand-alone motion kernel takes every step.
+bool step_kernel_walls(const EnvK& env) { return env.W <= MAXW; }
+
+// The environment without its walls, for rate kernels that read none: k_step MODE 0 and k_place_onehot then stage
+// nothing, whatever the wall count.
+EnvK without_walls(const EnvK& env) {
+  EnvK k = env;
+  k.walls = nullptr; k.W = 0; k.nb = 0; k.nh = 0; k.h0 = 0; k.aligned = 0;
+  return k;
 }
 
 int check_agents(const riab_agents* a) {
@@ -2132,7 +2157,12 @@ int launch_bvc(const EnvK& env, const riab_bvc_cells* bvc, const OutK& out, cons
   const size_t smemT = smemA + (size_t)bc.T * (sizeof(float2) + (size_t)env.W * sizeof(BvcTab));
   const bool table = env.W <= BVC_NW && smemT <= 40 * 1024;
   if (table) k_bvc_rays<true><<<(unsigned)n_tiles, NT, smemT, s>>>(env, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
-  else k_bvc_rays<false><<<(unsigned)n_tiles, NT, smemA, s>>>(env, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
+  else {
+    // the walls in float64 and float32 beside the directions: past 48 KB from about 950 walls at T = 180
+    const size_t smemW = smemA + (size_t)env.W * (4 * sizeof(double) + sizeof(float4));
+    if (smemW > 48 * 1024) RIAB_CUDA_OK(cudaFuncSetAttribute(k_bvc_rays<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemW));
+    k_bvc_rays<false><<<(unsigned)n_tiles, NT, smemW, s>>>(env, bc, pos_in, n_rows, scratch, first_wall, zsp, out.spike_ld);
+  }
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   if (pipe) {                                         // the integral (and its post-pass) go to the side stream
@@ -2547,6 +2577,7 @@ struct Pop {
   int kind = -1, n_cells = 0;
   int n_pad = 0;                        // the k_step kinds' packed cell count (a multiple of CELL_PAD), else 0
   bool step_policy = false;             // has_step_policy
+  bool walls = false;                   // its rate kernels read the walls (pop_reads_walls)
   double bound = -1.0;                  // an upper bound of the rates for thinned spikes (make_out), negative for none
   OutK out;
   PlaceConst place; GridConst grid; OvcConst ovc; KinConst kin; AvcConst avc; PppcConst pppc; PwnConst pwn;
@@ -2567,12 +2598,28 @@ bool has_step_policy(int kind, const void* cells) {
          kind == RIAB_CELLS_PPPC || kind == RIAB_CELLS_PWN;
 }
 
+// Whether a population's rate kernels read the walls: BVC rays (any wall count up to RIAB_MAX_WALLS), and the line of
+// sight / geodesic distances and occlusion tests, which k_step, k_place_onehot and k_rsn run over at most MAXW staged walls.
+bool pop_reads_walls(int kind, const void* cells) {
+  if (kind == RIAB_CELLS_BVC) return true;
+  if (kind == RIAB_CELLS_PLACE) return ((const riab_place_cells*)cells)->wall_geometry != RIAB_GEOM_EUCLIDEAN;
+  if (kind == RIAB_CELLS_PPPC) return ((const riab_pppc_cells*)cells)->place.wall_geometry != RIAB_GEOM_EUCLIDEAN;
+  if (kind == RIAB_CELLS_RSN) return ((const riab_rsn_cells*)cells)->points.wall_geometry != RIAB_GEOM_EUCLIDEAN;
+  if (kind == RIAB_CELLS_OVC) return ((const riab_ovc_cells*)cells)->walls_occlude != 0;
+  if (kind == RIAB_CELLS_AVC) return ((const riab_avc_cells*)cells)->walls_occlude != 0;
+  return false;
+}
+
 int make_pop(const EnvK& ek, int kind, const void* cells, const riab_rates_out* out, const riab_neuron_noise* noise,
              double dt, const riab_agents& ag, Pop& d) {
   if (cells == nullptr) return fail(RIAB_ERR_INVALID, "cells NULL");
   int rc = 0;
   d.kind = kind;
   d.step_policy = has_step_policy(kind, cells);
+  d.walls = pop_reads_walls(kind, cells);
+  if (d.walls && kind != RIAB_CELLS_BVC && ek.W > MAXW)
+    return fail(RIAB_ERR_UNSUPPORTED, "n_walls=%d: line_of_sight / geodesic distances and walls_occlude read at most %d walls "
+                "(wall_geometry=\"euclidean\" or walls_occlude=False read none and take up to %d)", ek.W, MAXW, RIAB_MAX_WALLS);
   if (kind == RIAB_CELLS_PLACE) {
     const riab_place_cells* pc = (const riab_place_cells*)cells;
     rc = make_place(pc, ek, d.place);
@@ -2635,8 +2682,10 @@ bool ffl_like(int kind) { return kind == RIAB_CELLS_FFL || kind == RIAB_CELLS_TD
 // (rates at the current positions while the motion of the next step runs, riab_run); 3 / 4: riab_run's whole run (run),
 // for the kinds whole_run_applies admits.  Kinds without a k_step policy run MODE 0 only.
 template <int MODE>
-int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const Pop& d,
+int launch_pop(const EnvK& env, const riab_agents& ag, const riab_motion_params& mp, const riab_step_io& io, const Pop& d,
                cudaStream_t s, BvcPipe* pipe = nullptr, const RunK* run = nullptr) {
+  // rates alone, of a population that reads no walls: stage none (MODE 1 - 4 also run the motion: step_kernel_walls)
+  const EnvK ek = (MODE == 0 && !d.walls) ? without_walls(env) : env;
   const double* pos_in = (MODE == 0 || MODE == 2) ? ag.pos : nullptr;
   const long long n = ag.n_agents;
   if (!d.step_policy) {
@@ -2673,14 +2722,14 @@ int launch_pop(const EnvK& ek, const riab_agents& ag, const riab_motion_params& 
 
 // The motion steps a rate kernel cannot take: parity taps (only the stand-alone motion kernel records them), and those of
 // populations without a k_step policy.
-bool needs_motion_kernel(const riab_step_io& io, const Pop& d) {
-  return io.collision_mask || io.first_hit || io.n_iters || !d.step_policy;
+bool needs_motion_kernel(const EnvK& ek, const riab_step_io& io, const Pop& d) {
+  return io.collision_mask || io.first_hit || io.n_iters || !d.step_policy || !step_kernel_walls(ek);
 }
 
 // One motion step, then population d's rates at the new positions; everything is checked before.
 int step_fused(const riab_agents* agents, const riab_env* env, const EnvK& ek, const riab_motion_params* prm,
                const riab_step_io* io, const Pop& d, cudaStream_t s, BvcPipe* pipe = nullptr) {
-  if (!needs_motion_kernel(*io, d)) return launch_pop<1>(ek, *agents, *prm, *io, d, s);
+  if (!needs_motion_kernel(ek, *io, d)) return launch_pop<1>(ek, *agents, *prm, *io, d, s);
   const int rc = riab_agent_update(agents, env, prm, io, s);
   return rc ? rc : launch_pop<0>(ek, *agents, kNoMotion, kNoStep, d, s, pipe);
 }
@@ -2793,7 +2842,7 @@ int whole_run_applies(const EnvK& ek, const riab_agents& ag, const riab_motion_p
                       const riab_motion_source* src, const riab_population* pops, int n_pops,
                       const riab_agent_history* hist, Pop& d, bool& yes) {
   yes = false;
-  if (n_pops != 1 || getenv("RIAB_NO_WHOLE_RUN") != nullptr || io.drift_velocity != nullptr || io.pos_mirror != nullptr ||
+  if (n_pops != 1 || !step_kernel_walls(ek) || getenv("RIAB_NO_WHOLE_RUN") != nullptr || io.drift_velocity != nullptr || io.pos_mirror != nullptr ||
       (src == nullptr && (io.xi != nullptr || io.collision_mask || io.first_hit || io.n_iters)))
     return 0;
   const riab_population& pp = pops[0];
@@ -2846,9 +2895,9 @@ int plan_run(const EnvK& ek, const riab_agents& ag, const riab_motion_params& pr
   // as the plain sequence, but the float64 motion chain never gates the rate warps.  A motion source keeps the plain
   // schedule (its motion kernel is cheap next to the rates).
   const bool skew = n_pops >= 1 && has_step_policy(pops[0].kind, pops[0].cells) && !any_ffl && io.xi == nullptr &&
-                    !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr;
+                    !io.collision_mask && !io.first_hit && !io.n_iters && src == nullptr && step_kernel_walls(ek);
   plan.sched = skew ? RunPlan::SKEWED : RunPlan::PLAIN;
-  plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || ffl_like(pops[0].kind));
+  plan.motion_alone = !skew && (src != nullptr || n_pops == 0 || ffl_like(pops[0].kind) || !step_kernel_walls(ek));
   // populations 1.. first (they read the positions of step st), population 0 last (it may advance them); then the
   // FeedForwardLayers in registration order, after every row they read of this step exists
   for (int p = skew ? 1 : 0; p < n_pops; ++p)
@@ -3021,7 +3070,8 @@ int hostio(HostIo*& h) {
 template <int KIND>
 __global__ void __launch_bounds__(128) k_subagent(const riab_subagent sa, const riab_motion_params mp, const MotionDerived md,
                                                   const EnvK env) {
-  __shared__ __align__(16) double s_walls[MAXW * 4];
+  extern __shared__ __align__(128) unsigned char dyn_sub[];           // env.W * 32 bytes of walls (none for a ShiftAgent)
+  double* s_walls = reinterpret_cast<double*>(dyn_sub);
   __shared__ uint64_t s_bar;
   if (KIND != RIAB_SUBAGENT_SHIFT) stage_walls(s_walls, &s_bar, env);
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -3209,8 +3259,9 @@ int riab_agent_update(const riab_agents* agents, const riab_env* env, const riab
   const bool rec = io->collision_mask || io->first_hit || io->n_iters;
   MotionDerived md;
   derive_motion(*prm, md);
-  if (rec) k_agent_update<true><<<grid, 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
-  else k_agent_update<false><<<grid, 128, 0, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
+  const size_t smem = motion_walls_bytes(ek);
+  if (rec) k_agent_update<true><<<grid, 128, smem, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
+  else k_agent_update<false><<<grid, 128, smem, (cudaStream_t)stream>>>(*agents, *prm, md, *io, ek);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;
@@ -3264,7 +3315,8 @@ int riab_agent_update_src(const riab_agents* agents, const riab_env* env, const 
 // (riab_theta.cuh).  Look-ahead steps advance the agent's forward rollout with motion_step in place.
 __global__ void __launch_bounds__(128) k_theta_seq(const riab_theta_seq ts, const riab_motion_params mp,
                                                    const MotionDerived md, const EnvK env) {
-  __shared__ __align__(16) double s_walls[MAXW * 4];
+  extern __shared__ __align__(128) unsigned char dyn_theta[];         // env.W * 32 bytes of walls
+  double* s_walls = reinterpret_cast<double*>(dyn_theta);
   __shared__ uint64_t s_bar;
   stage_walls(s_walls, &s_bar, env);
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -3366,7 +3418,7 @@ int riab_theta_seq_step(const riab_theta_seq* ts, const riab_env* env, const ria
   if (ts->xi_forward != nullptr && ts->xi_steps < 0) return fail(RIAB_ERR_INVALID, "xi_steps < 0");
   MotionDerived md;
   derive_motion(*fwd_prm, md);
-  k_theta_seq<<<(unsigned)((ts->n_agents + 127) / 128), 128, 0, (cudaStream_t)stream>>>(*ts, *fwd_prm, md, ek);
+  k_theta_seq<<<(unsigned)((ts->n_agents + 127) / 128), 128, motion_walls_bytes(ek), (cudaStream_t)stream>>>(*ts, *fwd_prm, md, ek);
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());
   return 0;
@@ -3387,10 +3439,10 @@ int riab_subagent_step(const riab_subagent* sa, const riab_env* env, const riab_
   riab_motion_params mp{};
   if (sa->kind == RIAB_SUBAGENT_SHIFT) {
     if (!sa->lead_head_direction) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL lead_head_direction");
-    k_subagent<RIAB_SUBAGENT_SHIFT><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, mp, md, ek);
+    k_subagent<RIAB_SUBAGENT_SHIFT><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, mp, md, ek);     // stages no walls
   } else if (sa->kind == RIAB_SUBAGENT_DUMB) {
     if (!sa->displacement || !sa->displacement_velocity) return fail(RIAB_ERR_INVALID, "riab_subagent_step: NULL displacement");
-    k_subagent<RIAB_SUBAGENT_DUMB><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, mp, md, ek);
+    k_subagent<RIAB_SUBAGENT_DUMB><<<grid, 128, motion_walls_bytes(ek), (cudaStream_t)stream>>>(*sa, mp, md, ek);
   } else {
     if (sham_prm == nullptr) return fail(RIAB_ERR_INVALID, "riab_subagent_step: a ReplayAgent needs sham_prm");
     if ((rc = check_motion(sham_prm))) return rc;
@@ -3400,7 +3452,7 @@ int riab_subagent_step(const riab_subagent* sa, const riab_env* env, const riab_
     if ((rc = check_agents(&sham))) return rc;
     if (sa->xi_replay != nullptr && sa->xi_steps < 0) return fail(RIAB_ERR_INVALID, "xi_steps < 0");
     derive_motion(*sham_prm, md);
-    k_subagent<RIAB_SUBAGENT_REPLAY><<<grid, 128, 0, (cudaStream_t)stream>>>(*sa, *sham_prm, md, ek);
+    k_subagent<RIAB_SUBAGENT_REPLAY><<<grid, 128, motion_walls_bytes(ek), (cudaStream_t)stream>>>(*sa, *sham_prm, md, ek);
   }
   g_launches++;
   RIAB_CUDA_OK(cudaGetLastError());

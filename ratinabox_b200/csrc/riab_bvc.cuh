@@ -81,18 +81,17 @@ RIAB_DEV BvcScreen bvc_screen(const float4 wl, float pxf, float pyf, float sapxf
 
 // The reference's float64 evaluation (utils.vector_intercepts, utils.py:74-97; preference Neurons.py:1763-1777) of the
 // walls in `mask`, in increasing wall order; np.argmax keeps the first maximum.
+// bvc_walk_bits: the walls w0 + (set bits of mask), carrying the running maximum (best, besti, best_la) so that
+// consecutive blocks of walls walk like one mask; bvc_walk_end: the result.
 template <typename MaskT>
-RIAB_DEV void bvc_walk(MaskT mask, double px, double py, double ux, double uy, const double* __restrict__ walls,
-                       double& dist, int& wall_id) {
+RIAB_DEV void bvc_walk_bits(MaskT mask, int w0, double px, double py, double ux, double uy, const double* __restrict__ walls,
+                            double& best, int& besti, double& best_la) {
   const D a0x(px), a0y(py);
   const D a1x = a0x + D(ux), a1y = a0y + D(uy);      // pos_line_segments[:, :, 1, :] += test_directions
   const D sax = a1x - a0x, say = a1y - a0y;
   const D sapx = -say, sapy = sax;
-  double best = -1.0;                                    // rejected walls all score -1
-  int besti = -1;
-  double best_la = 0.0;
   while (mask) {
-    const int w = (sizeof(MaskT) == 8) ? __ffsll((long long)mask) - 1 : __ffs((int)mask) - 1;
+    const int w = w0 + ((sizeof(MaskT) == 8) ? __ffsll((long long)mask) - 1 : __ffs((int)mask) - 1);
     mask &= mask - 1;
     const D bx0(walls[4 * w]), by0(walls[4 * w + 1]), bx1(walls[4 * w + 2]), by1(walls[4 * w + 3]);
     const D d0x = bx0 - a0x, d0y = by0 - a0y;
@@ -116,6 +115,12 @@ RIAB_DEV void bvc_walk(MaskT mask, double px, double py, double ux, double uy, c
     const double pref = (la > 0.0) ? __ddiv_rn(1.0, la) : ((la < 0.0) ? -1.0 : 0.0);
     if (pref > best) { best = pref; besti = w; best_la = la; }
   }
+}
+RIAB_DEV void bvc_walk_end(double px, double py, double ux, double uy, const double* __restrict__ walls, int besti,
+                           double best_la, double& dist, int& wall_id) {
+  const D a0x(px), a0y(py);
+  const D a1x = a0x + D(ux), a1y = a0y + D(uy);
+  const D sax = a1x - a0x, say = a1y - a0y;
   if (besti < 0) {
     // every wall scored -1: np.argmax returns wall 0, whose l_a is reported (Neurons.py:1677-1684)
     besti = 0;
@@ -127,6 +132,15 @@ RIAB_DEV void bvc_walk(MaskT mask, double px, double py, double ux, double uy, c
   }
   dist = best_la;
   wall_id = besti;
+}
+template <typename MaskT>
+RIAB_DEV void bvc_walk(MaskT mask, double px, double py, double ux, double uy, const double* __restrict__ walls,
+                       double& dist, int& wall_id) {
+  double best = -1.0;                                    // rejected walls all score -1
+  int besti = -1;
+  double best_la = 0.0;
+  bvc_walk_bits<MaskT>(mask, 0, px, py, ux, uy, walls, best, besti, best_la);
+  bvc_walk_end(px, py, ux, uy, walls, besti, best_la, dist, wall_id);
 }
 
 // Generic screen (any number of walls): everything from the float32 wall copies, per (ray, wall).
@@ -151,11 +165,37 @@ RIAB_DEV void bvc_first_wall_impl(double px, double py, double ux, double uy, co
   }
   bvc_walk<MaskT>(mask, px, py, ux, uy, walls, dist, wall_id);
 }
+// More than 64 walls: the same walls kept as bvc_first_wall_impl keeps -- those not rejected and not behind the final
+// bound, which is the minimum over every wall -- from a first pass for the bound and a second that screens and walks
+// blocks of 64 walls in increasing order.
+RIAB_DEV void bvc_first_wall_many(double px, double py, double ux, double uy, const double* __restrict__ walls,
+                                  const float4* __restrict__ wf, int W, float flo_env, double& dist, int& wall_id) {
+  const float pxf = (float)px, pyf = (float)py, sapxf = -(float)uy, sapyf = (float)ux;
+  const float flo = flo_env + flo_env * (fabsf(pxf) + fabsf(pyf));
+  float thr = INFINITY;
+  for (int w = 0; w < W; ++w) {
+    const BvcScreen sc = bvc_screen(wf[w], pxf, pyf, sapxf, sapyf, flo);
+    if (sc.lb_certain && sc.la_lo > 0.f) thr = fminf(thr, sc.la_hi);
+  }
+  double best = -1.0, best_la = 0.0;
+  int besti = -1;
+  for (int w0 = 0; w0 < W; w0 += 64) {
+    unsigned long long mask = 0;
+    const int n = (W - w0) < 64 ? (W - w0) : 64;
+    for (int j = 0; j < n; ++j) {
+      const BvcScreen sc = bvc_screen(wf[w0 + j], pxf, pyf, sapxf, sapyf, flo);
+      if (!(sc.lb_rejected || (sc.la_hi < 0.f) || (sc.la_lo > thr))) mask |= 1ull << j;
+    }
+    bvc_walk_bits<unsigned long long>(mask, w0, px, py, ux, uy, walls, best, besti, best_la);
+  }
+  bvc_walk_end(px, py, ux, uy, walls, besti, best_la, dist, wall_id);
+}
 // flo_env = 1e-6 * max(1, largest |coordinate| of a wall end) * (longest wall), see bvc_screen
 RIAB_DEV void bvc_first_wall(double px, double py, double ux, double uy, const double* __restrict__ walls,
                              const float4* __restrict__ wf, int W, float flo_env, double& dist, int& wall_id) {
   if (W <= 32) bvc_first_wall_impl<uint32_t>(px, py, ux, uy, walls, wf, W, flo_env, dist, wall_id);   // warp-uniform
-  else bvc_first_wall_impl<unsigned long long>(px, py, ux, uy, walls, wf, W, flo_env, dist, wall_id);
+  else if (W <= 64) bvc_first_wall_impl<unsigned long long>(px, py, ux, uy, walls, wf, W, flo_env, dist, wall_id);
+  else bvc_first_wall_many(px, py, ux, uy, walls, wf, W, flo_env, dist, wall_id);
 }
 
 // Table screen (at most BVC_NW walls).  A thread keeps ONE agent for all its test angles, so everything that depends on
